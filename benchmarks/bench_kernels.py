@@ -9,6 +9,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel det      # K1 variants
   python benchmarks/bench_kernels.py --kernel regrid   # K5, configs[3]
   python benchmarks/bench_kernels.py --kernel spectrum # K4, configs[4]
+  python benchmarks/bench_kernels.py --kernel climatology --steps 3
 """
 import argparse
 import json
@@ -325,15 +326,109 @@ def bench_threshold(args):
            'grid_cells')
 
 
+def _card():
+  """Card name and power limit of this run (a number depends on both)."""
+  import subprocess
+  import torch
+  info = {'card': torch.cuda.get_device_name(0)}
+  try:
+    info['power_limit_W'] = float(subprocess.run(
+        ['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader,nounits',
+         '-i', '0'], capture_output=True, text=True, timeout=30,
+        check=True).stdout.split()[0])
+  except Exception:  # pylint: disable=broad-except
+    info['power_limit_W'] = None
+  return info
+
+
+def climatology_bytes(nsel, ncell, nhour, nday, nstat, esize=4):
+  """Bytes the climatology needs: every selected time step of every cell read
+  once, every output written once.  The per-day moments stay in shared memory
+  (20 B per day slot and cell), so they add no HBM traffic."""
+  return nsel * ncell * esize + nstat * nhour * nday * ncell * 4
+
+
+def bench_climatology(args):
+  """Hourly explicit mean + std (scripts/compute_climatology.py's default
+  method) on a device-resident 721 x 1440 series (4 years 6-hourly, 24 GB)
+  and on a 13-level 121 x 240 series (5 years 6-hourly) streamed from host
+  memory."""
+  import time
+  import numpy as np
+  torch, _lib, ctx = setup()
+  from weatherbench2_b200 import utils
+  card = _card()
+  hours = [0, 6, 12, 18]
+  # device-resident
+  times = np.arange(np.datetime64('2017-01-01', 'ns'),
+                    np.datetime64('2021-01-01', 'ns'), np.timedelta64(6, 'h'))
+  ncell = NLAT * NLON
+  x = torch.empty((times.size, ncell), device='cuda', dtype=torch.float32)
+  for i in range(0, times.size, 512):
+    x[i:i + 512].normal_()
+  plan, labels = utils._plan(times, slice('2017', '2020'), hours,  # pylint: disable=protected-access
+                             utils.EXPLICIT, False, 61)
+  mean = torch.empty((len(hours), labels.size, ncell), device='cuda')
+  std = torch.empty_like(mean)
+  fn = lambda: ctx.climatology(x.data_ptr(), _lib.F32, times.size, ncell, plan,
+                               mean.data_ptr(), std.data_ptr())
+  ms = timeit(fn, args.steps, warmup=1)
+  nbytes = climatology_bytes(times.size, ncell, len(hours), labels.size, 2)
+  report('climatology device 721x1440 6-hourly 4y hourly explicit mean+std',
+         ms, nbytes, times.size * ncell, 'values', dict(
+             card, input_GB=times.size * ncell * 4 / 1e9))
+  del x, mean, std
+  torch.cuda.empty_cache()
+  # streamed from host memory
+  times = np.arange(np.datetime64('2016-01-01', 'ns'),
+                    np.datetime64('2021-01-01', 'ns'), np.timedelta64(6, 'h'))
+  ncell = 13 * 121 * 240
+  rs = np.random.default_rng(0)
+  block = rs.standard_normal((61, ncell), dtype=np.float32)
+  xh = np.empty((times.size, ncell), np.float32)
+  for i in range(0, times.size, 61):
+    xh[i:i + 61] = block[:times.size - i]
+  plan, labels = utils._plan(times, slice('2016', '2020'), hours,  # pylint: disable=protected-access
+                             utils.EXPLICIT, False, 61)
+  mh = np.empty((len(hours), labels.size, ncell), np.float32)
+  sh = np.empty_like(mh)
+  run = lambda: ctx.climatology_host(xh.ctypes.data, _lib.F32, times.size,
+                                     ncell, plan, utils.STREAM_BUDGET_BYTES,
+                                     mh.ctypes.data, sh.ctypes.data)
+  run()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    run()
+  s = (time.perf_counter() - t0) / args.steps
+  # the pageable host -> device rate of this machine, 1 GiB
+  probe = xh.reshape(-1)[:1 << 28]
+  dev = torch.empty(probe.size, device='cuda', dtype=torch.float32)
+  dev.copy_(torch.from_numpy(probe))
+  torch.cuda.synchronize()
+  t0 = time.perf_counter()
+  for _ in range(3):
+    dev.copy_(torch.from_numpy(probe))
+  torch.cuda.synchronize()
+  h2d = 3 * probe.nbytes / (time.perf_counter() - t0) / 1e9
+  nbytes = climatology_bytes(times.size, ncell, len(hours), labels.size, 2)
+  gbs = nbytes / s / 1e9
+  print(json.dumps(dict(
+      card, kernel='climatology streamed 13x121x240 6-hourly 5y hourly '
+      'explicit mean+std', ms=s * 1e3, algorithmic_GB=nbytes / 1e9,
+      achieved_GBps=gbs, h2d_pageable_GBps=h2d, frac_of_h2d=gbs / h2d)),
+        flush=True)
+
+
 if __name__ == '__main__':
   ap = argparse.ArgumentParser()
   ap.add_argument('--kernel', required=True,
                   choices=['ens', 'energy', 'det', 'regrid', 'spectrum',
-                           'maps', 'threshold'])
+                           'maps', 'threshold', 'climatology'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
   a = ap.parse_args()
   {'ens': bench_ens, 'energy': bench_energy, 'det': bench_det, 'regrid': bench_regrid,
    'spectrum': bench_spectrum, 'maps': bench_maps,
-   'threshold': bench_threshold}[a.kernel](a)
+   'threshold': bench_threshold,
+   'climatology': bench_climatology}[a.kernel](a)

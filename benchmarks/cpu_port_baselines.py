@@ -81,6 +81,21 @@ def main():
   s = timed(lambda: orc.zonal_energy_spectrum(xs, dims, lat, lon))
   out.append({'path': 'K4 zonal energy spectrum', 'sample': '13 x 721 x 1440',
               'seconds': s, 'grid_cells_per_s': xs.size / s})
+  # climatology: hourly explicit mean + std (compute_climatology.py's default
+  # method), 4 years 6-hourly, 64 cells of the 721 x 1440 grid
+  sys.path.insert(0, os.path.join(ROOT, 'tests'))
+  import climatology_oracle as co  # pylint: disable=import-outside-toplevel
+  times = np.arange(np.datetime64('2017-01-01', 'ns'),
+                    np.datetime64('2021-01-01', 'ns'), np.timedelta64(6, 'h'))
+  xc = rs.standard_normal((times.size, 64)).astype(np.float32)
+
+  def clim():
+    for stat in ('mean', 'std'):
+      co.hourly_stat(times, xc, 61, slice('2017', '2020'), 6, stat)
+  s = timed(clim, reps=1)
+  out.append({'path': 'climatology hourly explicit mean+std',
+              'sample': f'{times.size} 6-hourly steps x 64 cells',
+              'seconds': s, 'values_per_s': xc.size / s})
   for o in out:
     o.update({'cores': 1, 'kind': 'port'})
     print(json.dumps(o), flush=True)

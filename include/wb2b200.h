@@ -304,6 +304,54 @@ int wb2_spectrum_interp(wb2_ctx* ctx, const float* spec, int64_t nfield,
                         int32_t nrow, int32_t nk, const double* freq_table,
                         int32_t nfreq, const double* freqs, float* out);
 
+/* ---- day-of-year climatology --------------------------------------------------------
+ * wb2_climatology replaces compute_hourly_stat / compute_daily_stat (the
+ * `explicit` method, weatherbench2/utils.py:88-166) and compute_hourly_stat_fast
+ * / compute_daily_stat_fast (`fast`, utils.py:169-287) for the statistics mean
+ * and std of scripts/compute_climatology.py.  The series x is [time][ncell]
+ * (cells contiguous, float32 or float64); the host describes the selection:
+ *   nres > 0   x is first resampled to days: day i = skip-NaN mean of the
+ *              res_count[i] consecutive slabs from res_start[i] (host, NaN when
+ *              the count is 0; float32 input only), and the tables below index
+ *              those days instead of x's time steps
+ *   items      host [nhour][nday][nitem]: the steps feeding day slot d of hour h
+ *              (explicit: the value of stacked year j; fast: any step with that
+ *              day-of-year label), -1 = missing
+ *   fill       host [nhour][nitem]: the day-365 step of stacked year j (-1 =
+ *              none) that replaces a NaN / missing item (explicit only, else
+ *              ignored; utils.py:105)
+ *   hour_nday  host [nhour]: day slots of hour h, the period of the circular
+ *              window (the window wraps positionally over slots 0..n-1)
+ *   out_row    host [nhour][nday]: output row of each slot, < nday_out; rows an
+ *              hour does not produce are NaN
+ *   method     0 explicit: xarray's weighted mean / population std over (window,
+ *              year) with the triangular weights of create_window_weights
+ *              1 fast: per-slot mean / std (ddof 0), then the mean over the
+ *              window of weight * value, NaN skipped (count denominator)
+ *   mean, std  device [nhour][nday_out][ncell] float32; either may be NULL
+ * Moments accumulate in float64 around a per-cell shift; one read of x serves
+ * both statistics.  window_size: odd, >= 3.                                      */
+int wb2_climatology(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime,
+                    int64_t ncell, int64_t nres, const int64_t* res_start,
+                    const int32_t* res_count, int32_t nhour, int32_t nday,
+                    int32_t nitem, const int64_t* items, const int64_t* fill,
+                    const int32_t* hour_nday, const int32_t* out_row,
+                    int32_t nday_out, int32_t window_size, int32_t method,
+                    float* mean, float* std);
+
+/* wb2_climatology on a HOST series (NumPy / memmap): bands of cells, each band's
+ * selected time rows in one strided 2-D copy, double buffered so that the copy
+ * of band b+1 overlaps the kernels of band b.  `budget` bounds the device bytes
+ * of the two staging buffers (at least one cell per band).  mean / std are host
+ * [nhour][nday_out][ncell] float32.                                              */
+int wb2_climatology_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime,
+                         int64_t ncell, int64_t nres, const int64_t* res_start,
+                         const int32_t* res_count, int32_t nhour, int32_t nday,
+                         int32_t nitem, const int64_t* items, const int64_t* fill,
+                         const int32_t* hour_nday, const int32_t* out_row,
+                         int32_t nday_out, int32_t window_size, int32_t method,
+                         size_t budget, float* mean, float* std);
+
 /* ---- K10: rank histogram ---------------------------------------------------------
  * Replaces RankHistogram.compute_chunk (metrics.py:1894-2042) and the time mean
  * of EnsembleMetric.compute: rank of the truth among the members (NaN last),

@@ -63,6 +63,7 @@ _lib_lock = threading.Lock()
 
 _P = C.c_void_p
 _I64P = C.POINTER(C.c_int64)
+_I32P = C.POINTER(C.c_int32)
 
 # name -> (restype, argtypes); every symbol include/wb2b200.h declares
 PROTOTYPES = {
@@ -165,6 +166,14 @@ PROTOTYPES = {
                                                  C.c_int32,
                                                  C.POINTER(C.c_double), _P,
                                                  C.c_int64]),
+    'wb2_climatology': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, _I64P, _I32P,
+        C.c_int32, C.c_int32, C.c_int32, _I64P, _I64P, _I32P, _I32P, C.c_int32,
+        C.c_int32, C.c_int32, _P, _P]),
+    'wb2_climatology_host': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, _I64P, _I32P,
+        C.c_int32, C.c_int32, C.c_int32, _I64P, _I64P, _I32P, _I32P, C.c_int32,
+        C.c_int32, C.c_int32, C.c_size_t, _P, _P]),
 }
 
 
@@ -591,6 +600,34 @@ class Context:
         _as_ptr(step, C.c_double), int(fr.size), _as_ptr(fr, C.c_double),
         _P(out)))
 
+  # -- day-of-year climatology -----------------------------------------------
+  @staticmethod
+  def _climatology_args(plan: 'ClimatologyPlan'):
+    return (int(plan.nres), _as_ptr(plan.res_start, C.c_int64),
+            _as_ptr(plan.res_count, C.c_int32), int(plan.nhour),
+            int(plan.nday), int(plan.nitem), _as_ptr(plan.items, C.c_int64),
+            _as_ptr(plan.fill, C.c_int64), _as_ptr(plan.hour_nday, C.c_int32),
+            _as_ptr(plan.out_row, C.c_int32), int(plan.nday_out),
+            int(plan.window_size), int(plan.method))
+
+  def climatology(self, x: int, dtype: int, ntime: int, ncell: int,
+                  plan: 'ClimatologyPlan', mean: Optional[int],
+                  std: Optional[int]):
+    """x / mean / std are DEVICE addresses (wb2_climatology)."""
+    check(self.lib.wb2_climatology(
+        self.handle, _P(x), dtype, int(ntime), int(ncell),
+        *self._climatology_args(plan), _P(mean) if mean else None,
+        _P(std) if std else None))
+
+  def climatology_host(self, x: int, dtype: int, ntime: int, ncell: int,
+                       plan: 'ClimatologyPlan', budget: int,
+                       mean: Optional[int], std: Optional[int]):
+    """x / mean / std are HOST addresses (wb2_climatology_host)."""
+    check(self.lib.wb2_climatology_host(
+        self.handle, _P(x), dtype, int(ntime), int(ncell),
+        *self._climatology_args(plan), int(budget),
+        _P(mean) if mean else None, _P(std) if std else None))
+
   # -- K10 --------------------------------------------------------------------
   def rank_histogram(self, x: int, t: int, nmember: int, member_stride: int,
                      nout: int, ngroup: int, off_x: np.ndarray,
@@ -769,6 +806,32 @@ class WeightSpec:
     w.cell_w = self.cell_w_dev
     w.zero_skip = int(self.zero_skip)
     return w
+
+
+class ClimatologyPlan:
+  """Host-side owner of the index tables of wb2_climatology (see the header):
+  which time steps (or resampled days) feed every (hour, day slot)."""
+
+  def __init__(self, items, fill, hour_nday, out_row, nday_out, window_size,
+               method, res_start=None, res_count=None):
+    self.items = np.ascontiguousarray(items, dtype=np.int64)
+    self.nhour, self.nday, self.nitem = self.items.shape
+    self.fill = (np.ascontiguousarray(fill, dtype=np.int64)
+                 if fill is not None else np.full((self.nhour, self.nitem), -1,
+                                                  np.int64))
+    self.hour_nday = np.ascontiguousarray(hour_nday, dtype=np.int32)
+    self.out_row = np.ascontiguousarray(out_row, dtype=np.int32)
+    self.nday_out = int(nday_out)
+    self.window_size = int(window_size)
+    self.method = int(method)  # 0 explicit, 1 fast
+    if res_start is None:
+      self.res_start = np.zeros(1, np.int64)
+      self.res_count = np.zeros(1, np.int32)
+      self.nres = 0
+    else:
+      self.res_start = np.ascontiguousarray(res_start, dtype=np.int64)
+      self.res_count = np.ascontiguousarray(res_count, dtype=np.int32)
+      self.nres = int(self.res_start.size)
 
 
 class CsrSpec:

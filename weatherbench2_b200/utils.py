@@ -1,0 +1,306 @@
+"""Day-of-year climatologies (mean and standard deviation) on the GPU.
+
+Drop-in for the climatology functions of weatherbench2/utils.py and the
+computation of scripts/compute_climatology.py without Beam or zarr:
+
+  create_window_weights      utils.py:73-85
+  compute_hourly_stat        utils.py:143-166  (the `explicit` method)
+  compute_daily_stat         utils.py:127-140
+  compute_hourly_stat_fast   utils.py:217-272  (the `fast` method)
+  compute_daily_stat_fast    utils.py:200-214, 275-287
+  compute_climatology        compute_climatology.py:219-356 (`main`)
+
+The host turns the time selection into index tables (`_lib.ClimatologyPlan`):
+the reference's year stacking over the union of day-of-year labels
+(`xr.concat(dim='year')`, utils.py:97-103) or its `groupby('time.dayofyear')`.
+The CUDA kernel (csrc/climatology.cu) reads the (time, cells) series in place
+through them, accumulates float64 moments and applies the circular window.
+CUDA tensors stay on the device; NumPy arrays (np.memmap included) are streamed
+in bands of cells whose device footprint is bounded by `STREAM_BUDGET_BYTES`.
+
+Only the statistics 'mean' and 'std' are computed; the reference's 'seeps' and
+'quantile' climatologies are not (NotImplementedError).
+"""
+from __future__ import annotations
+
+from typing import Callable, Optional, Sequence, Union
+
+import numpy as np
+import pandas as pd
+
+from weatherbench2_b200 import _lib
+from weatherbench2_b200 import xarray_lite as xl
+
+EXPLICIT, FAST = 0, 1
+# device bytes of the two staging buffers of a NumPy input (one band of cells
+# each: its selected time rows, resampled days and outputs)
+STREAM_BUDGET_BYTES = 4 << 30
+
+StatFn = Union[str, Callable[..., object]]
+
+
+def create_window_weights(window_size: int) -> xl.DataArray:
+  """Triangular weights over `window_size` days, normalised to mean 1."""
+  assert window_size % 2 == 1, 'Window size must be odd.'
+  half = window_size // 2
+  w = np.concatenate([np.linspace(0, 1, half + 1),
+                      np.linspace(1, 0, half + 1)[1:]])
+  with np.errstate(invalid='ignore'):
+    w = w / w.mean()
+  return xl.DataArray(w, dims=['window'])
+
+
+def _check_window(window_size: int):
+  create_window_weights(window_size)  # AssertionError for an even size
+  if window_size < 3:
+    raise ValueError(f'window_size must be at least 3 (got {window_size}): '
+                     'the triangular weights of a 1-day window are 0 / 0')
+
+
+def _check_stat(stat_fn: StatFn):
+  if isinstance(stat_fn, str) and stat_fn in ('mean', 'std'):
+    return
+  raise NotImplementedError(
+      f'stat {stat_fn!r} not implemented: the GPU climatology computes the '
+      "statistics 'mean' and 'std'; the 'seeps' and 'quantile' statistics are "
+      'out of its scope')
+
+
+# -- index tables -------------------------------------------------------------
+def _select(times: pd.DatetimeIndex, clim_years) -> np.ndarray:
+  """Indices of `obs.sel(time=clim_years)` (label slice, partial strings)."""
+  if not isinstance(clim_years, slice):
+    raise TypeError(f'clim_years must be a slice, got {clim_years!r}')
+  start = None if clim_years.start is None else str(clim_years.start)
+  stop = None if clim_years.stop is None else str(clim_years.stop)
+  return np.arange(times.size)[times.slice_indexer(start, stop)]
+
+
+def _explicit_slots(times: pd.DatetimeIndex, idx: np.ndarray):
+  """Years stacked on the sorted union of their day-of-year labels; the fill
+  source of every year is its day-365 step (utils.py:97-105)."""
+  uy, yi = np.unique(np.asarray(times.year)[idx], return_inverse=True)
+  ud, di = np.unique(np.asarray(times.dayofyear)[idx], return_inverse=True)
+  if np.unique(di * uy.size + yi).size != idx.size:
+    raise ValueError('more than one time step per year and day of year')
+  items = np.full((ud.size, uy.size), -1, np.int64)
+  items[di, yi] = idx
+  pos = int(np.searchsorted(ud, 365))
+  if pos == ud.size or ud[pos] != 365:
+    raise KeyError(365)  # stacked.sel(dayofyear=365)
+  return ud, items, items[pos].copy()
+
+
+def _fast_slots(times: pd.DatetimeIndex, idx: np.ndarray):
+  """groupby('time.dayofyear'): every step of a label feeds its slot."""
+  ud, di = np.unique(np.asarray(times.dayofyear)[idx], return_inverse=True)
+  counts = np.bincount(di, minlength=ud.size)
+  order = np.argsort(di, kind='stable')
+  rank = np.arange(idx.size) - np.repeat(np.cumsum(counts) - counts, counts)
+  items = np.full((ud.size, int(counts.max())), -1, np.int64)
+  items[di[order], rank] = idx[order]
+  return ud, items, None
+
+
+def _daily_resample(times: pd.DatetimeIndex, idx: np.ndarray):
+  """resample(time='D'): every calendar day from the first to the last
+  selected step; day i averages `count[i]` consecutive steps from `start[i]`."""
+  ts = times[idx]
+  if not ts.is_monotonic_increasing or np.any(np.diff(idx) != 1):
+    raise ValueError('the daily resample needs a sorted time axis')
+  day = ts.floor('D')
+  days = pd.date_range(day[0], day[-1], freq='D')
+  k = np.asarray((day - days[0]) // pd.Timedelta(days=1), dtype=np.int64)
+  count = np.bincount(k, minlength=days.size).astype(np.int32)
+  start = np.zeros(days.size, np.int64)
+  start[k[::-1]] = idx[::-1]  # first step of each day
+  return days, start, count
+
+
+def _plan(times, clim_years, hours: Optional[Sequence[int]], method: int,
+          resample: bool, window_size: int):
+  """(ClimatologyPlan, day-of-year labels of the output)."""
+  times = pd.DatetimeIndex(times)
+  idx = _select(times, clim_years)
+  res = (None, None)
+  if resample:
+    if not idx.size:
+      raise ValueError(f'no time steps in {clim_years}')
+    times, start, count = _daily_resample(times, idx)
+    idx = np.arange(times.size)
+    res = (start, count)
+  slots = _explicit_slots if method == EXPLICIT else _fast_slots
+  per_hour = []
+  for hour in ([None] if hours is None else hours):
+    sel = idx if hour is None else idx[np.asarray(times.hour)[idx] == hour]
+    if not sel.size:  # the reference's xr.concat([]) / empty groupby
+      raise ValueError(f'no time steps at hour {hour} in {clim_years}')
+    per_hour.append(slots(times, sel))
+  labels = np.unique(np.concatenate([p[0] for p in per_hour]))
+  nhour = len(per_hour)
+  nday = max(p[0].size for p in per_hour)
+  nitem = max(p[1].shape[1] for p in per_hour)
+  items = np.full((nhour, nday, nitem), -1, np.int64)
+  fill = np.full((nhour, nitem), -1, np.int64)
+  hour_nday = np.zeros(nhour, np.int32)
+  out_row = np.zeros((nhour, nday), np.int32)
+  for h, (ud, it, fl) in enumerate(per_hour):
+    items[h, :ud.size, :it.shape[1]] = it
+    if fl is not None:
+      fill[h, :fl.size] = fl
+    hour_nday[h] = ud.size
+    out_row[h, :ud.size] = np.searchsorted(labels, ud)
+  plan = _lib.ClimatologyPlan(items, fill if method == EXPLICIT else None,
+                              hour_nday, out_row, labels.size, window_size,
+                              method, *res)
+  return plan, labels
+
+
+# -- execution ------------------------------------------------------------------
+def _run(ds: xl.Dataset, plan, labels, hours, stats: Sequence[str]) -> dict:
+  """{stat: {variable: DataArray}} for every variable with a time axis."""
+  ctx = _lib.default_context()
+  out = {s: {} for s in stats}
+  for name, da in ds.items():
+    if 'time' not in da.dims:
+      continue
+    ti = da.dims.index('time')
+    other = tuple(d for d in da.dims if d != 'time')
+    oshape = tuple(da.sizes[d] for d in other)
+    ncell = int(np.prod(oshape)) if oshape else 1
+    ntime = da.sizes['time']
+    nrow = (plan.nhour, plan.nday_out)
+    data = da.data
+    if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
+      import torch  # pylint: disable=import-outside-toplevel
+      x = data.movedim(ti, 0)
+      if x.dtype != torch.float64 or plan.nres:
+        x = x.to(torch.float32)
+      x = x.contiguous()
+      res = {s: torch.empty(nrow + oshape, device=x.device,
+                            dtype=torch.float32) for s in stats}
+      ptr = {s: res[s].data_ptr() if s in res else None for s in ('mean', 'std')}
+      ctx.climatology(x.data_ptr(),
+                      _lib.F64 if x.dtype == torch.float64 else _lib.F32,
+                      ntime, ncell, plan, ptr['mean'], ptr['std'])
+    else:
+      x = np.asarray(data)
+      if ti:
+        x = np.moveaxis(x, ti, 0)
+      dt = np.float64 if x.dtype == np.float64 and not plan.nres else np.float32
+      x = np.ascontiguousarray(x, dtype=dt)
+      res = {s: ctx.pinned_result(nrow + oshape, np.float32) for s in stats}
+      ptr = {s: res[s].ctypes.data if s in res else None
+             for s in ('mean', 'std')}
+      ctx.climatology_host(x.ctypes.data,
+                           _lib.F64 if dt == np.float64 else _lib.F32, ntime,
+                           ncell, plan, STREAM_BUDGET_BYTES, ptr['mean'],
+                           ptr['std'])
+    coords = {k: c for k, c in da.coords.items() if 'time' not in c.dims}
+    coords['dayofyear'] = xl.Coord(('dayofyear',), labels)
+    if hours is None:
+      dims = ('dayofyear',) + other
+      res = {s: v.reshape(nrow[1:] + oshape) for s, v in res.items()}
+    else:
+      dims = ('hour', 'dayofyear') + other
+      coords['hour'] = xl.Coord(('hour',), np.asarray(hours))
+    for s in stats:
+      out[s][name] = xl.DataArray(res[s], dims, coords, name, da.attrs)
+  return out
+
+
+def _compute(obs, window_size: int, clim_years: slice,
+             hours: Optional[Sequence[int]], method: int,
+             stats: Sequence[str]) -> dict:
+  """{stat: lite Dataset}; the daily fast mean averages the raw steps, every
+  other daily statistic the daily resample (utils.py:200-214)."""
+  _check_window(window_size)
+  for s in stats:
+    _check_stat(s)
+  ds = xl.from_xarray(obs)
+  times = ds.coords['time'].values
+  groups = [(list(stats), hours is None and method == EXPLICIT)]
+  if hours is None and method == FAST:
+    groups = [([s], s == 'std') for s in stats]
+  out = {}
+  for group, resample in groups:
+    plan, labels = _plan(times, clim_years, hours, method, resample,
+                         window_size)
+    for s, variables in _run(ds, plan, labels, hours, group).items():
+      out[s] = xl.Dataset(variables, attrs=ds.attrs)
+  return out
+
+
+def _public(obs, result: xl.Dataset):
+  return xl.to_xarray(result) if xl.is_native_xarray(obs) else result
+
+
+def _hours(hour_interval: int):
+  return list(range(0, 24, hour_interval))
+
+
+def compute_hourly_stat(obs, window_size: int, clim_years: slice,
+                        hour_interval: int, stat_fn: StatFn = 'mean'):
+  """Climatology by hour of day and day of year, `explicit` method."""
+  _check_stat(stat_fn)
+  res = _compute(obs, window_size, clim_years, _hours(hour_interval), EXPLICIT,
+                 [stat_fn])
+  return _public(obs, res[stat_fn])
+
+
+def compute_daily_stat(obs, window_size: int, clim_years: slice,
+                       stat_fn: StatFn = 'mean'):
+  """Climatology by day of year of the daily means, `explicit` method."""
+  _check_stat(stat_fn)
+  res = _compute(obs, window_size, clim_years, None, EXPLICIT, [stat_fn])
+  return _public(obs, res[stat_fn])
+
+
+def compute_hourly_stat_fast(obs, window_size: int, clim_years: slice,
+                             hour_interval: int, stat_fn: str = 'mean'):
+  """Per-day mean / std by hour of day, smoothed over the window (`fast`)."""
+  _check_stat(stat_fn)
+  res = _compute(obs, window_size, clim_years, _hours(hour_interval), FAST,
+                 [stat_fn])
+  return _public(obs, res[stat_fn])
+
+
+def compute_daily_stat_fast(obs, window_size: int, clim_years: slice,
+                            stat_fn: str = 'mean'):
+  """Per-day mean (raw steps) / std (daily means), smoothed (`fast`)."""
+  _check_stat(stat_fn)
+  res = _compute(obs, window_size, clim_years, None, FAST, [stat_fn])
+  return _public(obs, res[stat_fn])
+
+
+def compute_climatology(obs, *, frequency: str = 'hourly',
+                        hour_interval: int = 1, window_size: int = 61,
+                        start_year: int = 1990, end_year: int = 2020,
+                        statistics: Sequence[str] = ('mean',),
+                        method: str = 'explicit'):
+  """scripts/compute_climatology.py without Beam or zarr: variables without a
+  time axis are dropped, time is selected over [start_year, end_year] (both
+  inclusive), the mean keeps the variable's name and the std is `<var>_std`.
+  Dims (hour, dayofyear, ...) for hourly, (dayofyear, ...) for daily; the day
+  axis holds the day-of-year labels present in the selection.  Mean and std
+  are computed from one read of the data."""
+  stats = [statistics] if isinstance(statistics, str) else list(statistics)
+  for s in stats:
+    _check_stat(s)
+  if frequency not in ('hourly', 'daily'):
+    raise NotImplementedError(f'Frequency {frequency} not implemented.')
+  if method not in ('explicit', 'fast'):
+    raise NotImplementedError(
+        f'method {method} for climatological frequency {frequency} not '
+        'implemented.')
+  hours = _hours(hour_interval) if frequency == 'hourly' else None
+  res = _compute(obs, window_size, slice(str(start_year), str(end_year)),
+                 hours, EXPLICIT if method == 'explicit' else FAST, stats)
+  ds = xl.from_xarray(obs)
+  out = xl.Dataset(attrs=ds.attrs)
+  for s in stats:
+    for name, da in res[s].items():
+      key = name if s == 'mean' else f'{name}_{s}'
+      da.name = key
+      out[key] = da
+  return _public(obs, out)
