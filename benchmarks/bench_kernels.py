@@ -10,6 +10,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel regrid   # K5, configs[3]
   python benchmarks/bench_kernels.py --kernel spectrum # K4, configs[4]
   python benchmarks/bench_kernels.py --kernel climatology --steps 3
+  python benchmarks/bench_kernels.py --kernel climatology_quantile --steps 2
 """
 import argparse
 import json
@@ -419,11 +420,86 @@ def bench_climatology(args):
         flush=True)
 
 
+def bench_climatology_quantile(args):
+  """Hourly explicit quantiles (0.1, 0.25, 0.5, 0.75, 0.9) and the SEEPS pair
+  of a 121 x 240 field, 6-hourly 1990-2019 (5.1 GB), window 61: on the device
+  and streamed from host memory.  Bytes: every selected step read once, every
+  output written once.  Work: the sorted-window entries each output day's
+  prefix pass scans, nyear * (window - 2) per (hour, day, cell)."""
+  import time
+  import numpy as np
+  torch, _lib, ctx = setup()
+  from weatherbench2_b200 import utils
+  card = _card()
+  hours, qs, window = [0, 6, 12, 18], [0.1, 0.25, 0.5, 0.75, 0.9], 61
+  times = np.arange(np.datetime64('1990-01-01', 'ns'),
+                    np.datetime64('2020-01-01', 'ns'), np.timedelta64(6, 'h'))
+  ncell = 121 * 240
+  plan, labels = utils._plan(times, slice('1990', '2019'), hours,  # pylint: disable=protected-access
+                             utils.EXPLICIT, False, window)
+  entries = len(hours) * labels.size * ncell * plan.nitem * (window - 2)
+  x = torch.empty((times.size, ncell), device='cuda', dtype=torch.float32)
+  gen = torch.Generator(device='cuda').manual_seed(0)
+  for i in range(0, times.size, 4096):
+    x[i:i + 4096].normal_(generator=gen)
+  out = torch.empty((len(hours), len(qs), labels.size, ncell), device='cuda')
+  fn = lambda: ctx.climatology_quantile(x.data_ptr(), _lib.F32, times.size,
+                                        ncell, plan, qs, None, out.data_ptr(),
+                                        None)
+  ms = timeit(fn, args.steps, warmup=1)
+  nbytes = climatology_bytes(times.size, ncell, len(hours), labels.size,
+                             len(qs))
+  report('climatology_quantile device 121x240 6-hourly 30y hourly window 61 '
+         '5 quantiles', ms, nbytes, entries, 'window_entries',
+         dict(card, input_GB=times.size * ncell * 4 / 1e9))
+  # SEEPS on a precipitation-like field: about 40 % zeros
+  wet = torch.empty_like(x)
+  for i in range(0, times.size, 4096):
+    wet[i:i + 4096].uniform_(generator=gen)
+  x.abs_().mul_(1e-3).mul_((wet >= 0.4).float())
+  del wet
+  dry = torch.empty((len(hours), labels.size, ncell), device='cuda')
+  fn = lambda: ctx.climatology_quantile(x.data_ptr(), _lib.F32, times.size,
+                                        ncell, plan, [2 / 3], 0.25e-3,
+                                        out.data_ptr(), dry.data_ptr())
+  ms = timeit(fn, args.steps, warmup=1)
+  nbytes = climatology_bytes(times.size, ncell, len(hours), labels.size, 2)
+  report('climatology_quantile device 121x240 6-hourly 30y hourly window 61 '
+         'SEEPS (40% zeros)', ms, nbytes, entries, 'window_entries',
+         dict(card, note='window_entries counts every sample; dry ones '
+              'never enter the window'))
+  # the first workload from host memory
+  del x, out, dry
+  block = np.random.default_rng(1).standard_normal((4096, ncell),
+                                                    dtype=np.float32)
+  xh = np.empty((times.size, ncell), np.float32)
+  for i in range(0, times.size, 4096):
+    xh[i:i + 4096] = block[:times.size - i]
+  torch.cuda.empty_cache()
+  oh = np.empty((len(hours), len(qs), labels.size, ncell), np.float32)
+  run = lambda: ctx.climatology_quantile_host(
+      xh.ctypes.data, _lib.F32, times.size, ncell, plan, qs, None,
+      utils.STREAM_BUDGET_BYTES, oh.ctypes.data, None)
+  run()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    run()
+  s = (time.perf_counter() - t0) / args.steps
+  nbytes = climatology_bytes(times.size, ncell, len(hours), labels.size,
+                             len(qs))
+  print(json.dumps(dict(
+      card, kernel='climatology_quantile streamed 121x240 6-hourly 30y hourly '
+      'window 61 5 quantiles', ms=s * 1e3, algorithmic_GB=nbytes / 1e9,
+      achieved_GBps=nbytes / s / 1e9, window_entries_per_s=entries / s)),
+        flush=True)
+
+
 if __name__ == '__main__':
   ap = argparse.ArgumentParser()
   ap.add_argument('--kernel', required=True,
                   choices=['ens', 'energy', 'det', 'regrid', 'spectrum',
-                           'maps', 'threshold', 'climatology'])
+                           'maps', 'threshold', 'climatology',
+                           'climatology_quantile'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -431,4 +507,5 @@ if __name__ == '__main__':
   {'ens': bench_ens, 'energy': bench_energy, 'det': bench_det, 'regrid': bench_regrid,
    'spectrum': bench_spectrum, 'maps': bench_maps,
    'threshold': bench_threshold,
-   'climatology': bench_climatology}[a.kernel](a)
+   'climatology': bench_climatology,
+   'climatology_quantile': bench_climatology_quantile}[a.kernel](a)

@@ -352,6 +352,49 @@ int wb2_climatology_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime,
                          int32_t nday_out, int32_t window_size, int32_t method,
                          size_t budget, float* mean, float* std);
 
+/* wb2_climatology_quantile replaces Quantile.compute and SEEPSThreshold.compute
+ * (scripts/compute_climatology.py:130-177) passed as stat_fn to
+ * compute_hourly_stat / compute_daily_stat (weatherbench2/utils.py:88-166), the
+ * `explicit` method only.  The series and the tables are those of
+ * wb2_climatology (method 0, `fill` required).  Per output value the samples are
+ * the nyear x window_size entries of the wrapped window, the day-365 fill
+ * applied, tap j weighted by create_window_weights (utils.py:73-85), and the
+ * statistic is xarray's weighted type-7 quantile over (window, year): NaN and
+ * zero-weight samples dropped, nw = (sum w)^2 / sum w^2, c = [0, cumsum(w/sum w)]
+ * over the sorted values, h = clip((nw-1) q + 1, 1, nw),
+ * v = max((h-1)/nw, min(h/nw, c)) nw - h + 1, result sum_i x_i (v[i+1] - v[i]),
+ * NaN without samples.
+ *   quantiles  host [nquantile] in [0, 1], 1 <= nquantile <= 16
+ *   seeps      0: out = the quantiles, dry_fraction must be NULL
+ *              1: samples x < dry_threshold (compared in the series' precision)
+ *                 are dropped like NaN before the quantiles, and dry_fraction =
+ *                 the unweighted mean of (x < dry_threshold) over all
+ *                 nyear * window_size samples (NaN is not dry); SEEPSThreshold
+ *                 is nquantile 1, quantiles {2/3}
+ *   out        device [nhour][nquantile][nday_out][ncell] float32
+ *   dry_fraction  device [nhour][nday_out][ncell] float32 (seeps 1)
+ * nitem * window_size <= 8192.                                                   */
+int wb2_climatology_quantile(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime,
+                             int64_t ncell, int64_t nres, const int64_t* res_start,
+                             const int32_t* res_count, int32_t nhour, int32_t nday,
+                             int32_t nitem, const int64_t* items, const int64_t* fill,
+                             const int32_t* hour_nday, const int32_t* out_row,
+                             int32_t nday_out, int32_t window_size, int32_t nquantile,
+                             const double* quantiles, int32_t seeps, double dry_threshold,
+                             float* out, float* dry_fraction);
+
+/* wb2_climatology_quantile on a HOST series, streamed in bands of cells like
+ * wb2_climatology_host; out / dry_fraction are host arrays of the same layout. */
+int wb2_climatology_quantile_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime,
+                                  int64_t ncell, int64_t nres, const int64_t* res_start,
+                                  const int32_t* res_count, int32_t nhour, int32_t nday,
+                                  int32_t nitem, const int64_t* items, const int64_t* fill,
+                                  const int32_t* hour_nday, const int32_t* out_row,
+                                  int32_t nday_out, int32_t window_size, int32_t nquantile,
+                                  const double* quantiles, int32_t seeps,
+                                  double dry_threshold, size_t budget, float* out,
+                                  float* dry_fraction);
+
 /* ---- K10: rank histogram ---------------------------------------------------------
  * Replaces RankHistogram.compute_chunk (metrics.py:1894-2042) and the time mean
  * of EnsembleMetric.compute: rank of the truth among the members (NaN last),

@@ -174,7 +174,20 @@ PROTOTYPES = {
         _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, _I64P, _I32P,
         C.c_int32, C.c_int32, C.c_int32, _I64P, _I64P, _I32P, _I32P, C.c_int32,
         C.c_int32, C.c_int32, C.c_size_t, _P, _P]),
+    'wb2_climatology_quantile': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, _I64P, _I32P,
+        C.c_int32, C.c_int32, C.c_int32, _I64P, _I64P, _I32P, _I32P, C.c_int32,
+        C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_int32, C.c_double, _P,
+        _P]),
+    'wb2_climatology_quantile_host': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, _I64P, _I32P,
+        C.c_int32, C.c_int32, C.c_int32, _I64P, _I64P, _I32P, _I32P, C.c_int32,
+        C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_int32, C.c_double,
+        C.c_size_t, _P, _P]),
 }
+# wb2_climatology_quantile: quantiles per call, nitem * window_size per window
+CLIM_MAX_QUANTILES = 16
+CLIM_QUANTILE_MAX_SAMPLES = 8192
 
 
 def load_library():
@@ -627,6 +640,39 @@ class Context:
         self.handle, _P(x), dtype, int(ntime), int(ncell),
         *self._climatology_args(plan), int(budget),
         _P(mean) if mean else None, _P(std) if std else None))
+
+  @staticmethod
+  def _quantile_args(quantiles, seeps_threshold: Optional[float]):
+    q = np.ascontiguousarray(quantiles, dtype=np.float64)
+    return (int(q.size), _as_ptr(q, C.c_double),
+            int(seeps_threshold is not None),
+            float(seeps_threshold if seeps_threshold is not None else 0.0)), q
+
+  def climatology_quantile(self, x: int, dtype: int, ntime: int, ncell: int,
+                           plan: 'ClimatologyPlan', quantiles,
+                           seeps_threshold: Optional[float], out: int,
+                           dry_fraction: Optional[int]):
+    """x / out / dry_fraction are DEVICE addresses (wb2_climatology_quantile);
+    seeps_threshold None computes the quantiles, else the SEEPS pair."""
+    args, keep = self._quantile_args(quantiles, seeps_threshold)
+    check(self.lib.wb2_climatology_quantile(
+        self.handle, _P(x), dtype, int(ntime), int(ncell),
+        *self._climatology_args(plan)[:-1], *args, _P(out),
+        _P(dry_fraction) if dry_fraction else None))
+    del keep
+
+  def climatology_quantile_host(self, x: int, dtype: int, ntime: int,
+                                ncell: int, plan: 'ClimatologyPlan', quantiles,
+                                seeps_threshold: Optional[float], budget: int,
+                                out: int, dry_fraction: Optional[int]):
+    """x / out / dry_fraction are HOST addresses
+    (wb2_climatology_quantile_host)."""
+    args, keep = self._quantile_args(quantiles, seeps_threshold)
+    check(self.lib.wb2_climatology_quantile_host(
+        self.handle, _P(x), dtype, int(ntime), int(ncell),
+        *self._climatology_args(plan)[:-1], *args, int(budget), _P(out),
+        _P(dry_fraction) if dry_fraction else None))
+    del keep
 
   # -- K10 --------------------------------------------------------------------
   def rank_histogram(self, x: int, t: int, nmember: int, member_stride: int,

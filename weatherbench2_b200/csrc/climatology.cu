@@ -36,7 +36,7 @@
 
 #include <algorithm>
 
-#include "common.cuh"
+#include "climatology.cuh"
 
 namespace wb2 {
 
@@ -44,20 +44,6 @@ constexpr int kClimCells = 8;   // cells per CTA
 constexpr int kClimLanes = 32;  // day lanes per CTA
 constexpr int kClimThreads = kClimCells * kClimLanes;
 constexpr int kClimMaxDays = 1400;  // shared memory: 160 B per day slot
-
-struct ClimArgs {
-  const int64_t* items;      // [nhour][nday][nitem] time step (of the read series) or -1
-  const int64_t* fill;       // [nhour][nitem] day-365 step of stacked year j, or NULL
-  const int32_t* hour_nday;  // [nhour] day slots of this hour (the wrap period)
-  const int32_t* out_row;    // [nhour][nday] output row of each day slot
-  int64_t ncell;             // cells of this launch
-  int64_t tstride;           // elements between consecutive time steps
-  int64_t out_stride;        // elements between output rows
-  int32_t nhour, nday, nitem, nday_out, half;
-  int32_t fast;
-  float* mean;  // [nhour][nday_out][out_stride] or NULL
-  float* std;
-};
 
 __device__ __forceinline__ int wrap_day(int i, int n) {
   i %= n;
@@ -197,20 +183,7 @@ __global__ void __launch_bounds__(kClimThreads) climatology_kernel(const T* __re
   }
 }
 
-// The caller's tables, validated, in one device block.
-struct ClimPlan {
-  int64_t nres = 0;
-  const int64_t* res_start = nullptr;  // host
-  const int32_t* res_count = nullptr;  // host
-  int32_t nhour = 0, nday = 0, nitem = 0, nday_out = 0, half = 0, fast = 0;
-  const int64_t* items = nullptr;  // host
-  const int64_t* fill = nullptr;
-  const int32_t* hour_nday = nullptr;
-  const int32_t* out_row = nullptr;
-  bool need_nan_fill = false;  // some hour lacks some output day
-};
-
-static int clim_validate(int64_t ntime, int64_t nres, const int64_t* res_start,
+int clim_validate(int64_t ntime, int64_t nres, const int64_t* res_start,
                          const int32_t* res_count, int32_t nhour, int32_t nday, int32_t nitem,
                          const int64_t* items, const int64_t* fill, const int32_t* hour_nday,
                          const int32_t* out_row, int32_t nday_out, int32_t window_size,
@@ -271,15 +244,10 @@ static int clim_validate(int64_t ntime, int64_t nres, const int64_t* res_start,
   return WB2_OK;
 }
 
-// Device copy of the tables: [items][fill][hour_nday][out_row] in one block
-// (a Packer slot could be recycled by the wb2_ens_mean calls of the resample).
-struct ClimDeviceTables {
-  char* base = nullptr;
-  ClimArgs args{};
-};
-
-static int clim_upload(wb2_ctx* ctx, const ClimPlan& p, const int64_t* items,
-                       const int64_t* fill, ClimDeviceTables* t) {
+// One device block (a Packer slot could be recycled by the wb2_ens_mean calls
+// of the resample).
+int clim_upload(wb2_ctx* ctx, const ClimPlan& p, const int64_t* items, const int64_t* fill,
+                ClimDeviceTables* t) {
   const size_t n_items = size_t(p.nhour) * p.nday * p.nitem;
   const size_t n_fill = p.fill ? size_t(p.nhour) * p.nitem : 0;
   const size_t o_fill = n_items * 8;
@@ -310,8 +278,8 @@ static int clim_upload(wb2_ctx* ctx, const ClimPlan& p, const int64_t* items,
 
 // resample(time='D').mean(): day i is the skip-NaN mean of `count[i]`
 // consecutive time slabs from `start[i]` (NaN for a day without data).
-static int clim_resample(wb2_ctx* ctx, const float* x, int64_t tstride, int64_t ncell,
-                         const ClimPlan& p, const int64_t* start, float* daily) {
+int clim_resample(wb2_ctx* ctx, const float* x, int64_t tstride, int64_t ncell,
+                  const ClimPlan& p, const int64_t* start, float* daily) {
   int64_t i = 0;
   std::vector<int64_t> off;
   while (i < p.nres) {
@@ -356,6 +324,122 @@ static int clim_launch(wb2_ctx* ctx, const void* x, int dtype, int64_t ncell, in
   WB2_CUDA_TRY(cudaGetLastError());
   ctx->launches += 1;
   return WB2_OK;
+}
+
+int clim_stream_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime, int64_t ncell,
+                     const ClimPlan& p, size_t budget, int nout, float* const* out_host,
+                     const size_t* out_rows, const ClimBandFn& band) {
+  const size_t esize = dtype == WB2_F32 ? 4 : 8;
+  const int32_t nhour = p.nhour, nday = p.nday, nitem = p.nitem;
+  const int64_t nres = p.nres;
+  const int64_t* res_start = p.res_start;
+  const int32_t* res_count = p.res_count;
+  const int64_t* items = p.items;
+
+  // the time rows the selection touches; tables rebased to the first of them
+  int64_t t_lo = ntime, t_hi = -1;
+  const size_t n_items = size_t(nhour) * nday * nitem;
+  const size_t n_fill = p.fill ? size_t(nhour) * nitem : 0;
+  if (nres > 0) {
+    for (int64_t i = 0; i < nres; ++i)
+      if (res_count[i] > 0) {
+        t_lo = std::min(t_lo, res_start[i]);
+        t_hi = std::max(t_hi, res_start[i] + res_count[i] - 1);
+      }
+  } else {
+    for (size_t i = 0; i < n_items; ++i)
+      if (items[i] >= 0) t_lo = std::min(t_lo, items[i]), t_hi = std::max(t_hi, items[i]);
+    for (size_t i = 0; i < n_fill; ++i)
+      if (p.fill[i] >= 0) t_lo = std::min(t_lo, p.fill[i]), t_hi = std::max(t_hi, p.fill[i]);
+  }
+  const int64_t rows = t_hi >= t_lo ? t_hi - t_lo + 1 : 0;
+  if (rows == 0) t_lo = 0;
+  std::vector<int64_t> it_r(items, items + n_items), fill_r, start_r;
+  if (nres > 0) {
+    start_r.assign(res_start, res_start + nres);
+    for (auto& v : start_r) v -= t_lo;
+  } else {
+    for (auto& v : it_r)
+      if (v >= 0) v -= t_lo;
+  }
+  if (n_fill) {
+    fill_r.assign(p.fill, p.fill + n_fill);
+    if (nres == 0)
+      for (auto& v : fill_r)
+        if (v >= 0) v -= t_lo;
+  }
+
+  // band of cells: input rows + resampled days + outputs, double buffered
+  size_t out_per_cell = 0;
+  for (int s = 0; s < nout; ++s) out_per_cell += out_rows[s] * 4;
+  const size_t per_cell = size_t(rows) * esize + size_t(nres) * 4 + out_per_cell;
+  int64_t nb = static_cast<int64_t>(budget / (2 * per_cell));
+  nb = std::max<int64_t>(1, std::min(nb, ncell));
+  auto al = [](size_t b) { return (b + 255) / 256 * 256; };
+  const size_t b_in = al(size_t(rows) * nb * esize), b_day = al(size_t(nres) * nb * 4);
+  std::vector<size_t> b_out(static_cast<size_t>(nout));
+  size_t stage_bytes = b_in + b_day;
+  for (int s = 0; s < nout; ++s) stage_bytes += b_out[size_t(s)] = al(out_rows[s] * nb * 4);
+
+  ClimDeviceTables t;
+  char* stage[2] = {nullptr, nullptr};
+  const int rc = [&]() -> int {
+    WB2_TRY(clim_upload(ctx, p, it_r.data(), n_fill ? fill_r.data() : nullptr, &t));
+    for (int i = 0; i < 2; ++i)
+      WB2_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&stage[i]), stage_bytes));
+    const char* xh = static_cast<const char*>(x);
+    bool used[2] = {false, false};
+    int buf = 0;
+    std::vector<float*> out(static_cast<size_t>(nout));
+    for (int64_t c0 = 0; c0 < ncell; c0 += nb) {
+      const int64_t n = std::min(nb, ncell - c0);
+      char* in = stage[buf];
+      float* daily = reinterpret_cast<float*>(in + b_in);
+      char* o = in + b_in + b_day;
+      for (int s = 0; s < nout; ++s) {
+        out[size_t(s)] = reinterpret_cast<float*>(o);
+        o += b_out[size_t(s)];
+      }
+      if (used[buf])
+        WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
+      if (rows > 0) {  // the band's whole selected series: one strided 2-D copy
+        WB2_CUDA_TRY(cudaMemcpy2DAsync(in, size_t(n) * esize,
+                                       xh + (size_t(t_lo) * ncell + c0) * esize,
+                                       size_t(ncell) * esize, size_t(n) * esize, size_t(rows),
+                                       cudaMemcpyHostToDevice, ctx->copy_stream));
+        ctx->stat_h2d_bytes += rows * n * int64_t(esize);
+      }
+      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
+      WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
+      const void* src = in;
+      if (nres > 0) {
+        WB2_TRY(clim_resample(ctx, reinterpret_cast<const float*>(in), n, n, p, start_r.data(),
+                              daily));
+        src = daily;
+      }
+      if (p.need_nan_fill)
+        WB2_CUDA_TRY(cudaMemsetAsync(out[0], 0xFF, size_t(o - reinterpret_cast<char*>(out[0])),
+                                     ctx->stream));
+      WB2_TRY(band(src, n, t.args, out.data()));
+      for (int s = 0; s < nout; ++s) {
+        WB2_CUDA_TRY(cudaMemcpy2DAsync(out_host[s] + c0, size_t(ncell) * 4, out[size_t(s)],
+                                       size_t(n) * 4, size_t(n) * 4, out_rows[s],
+                                       cudaMemcpyDeviceToHost, ctx->stream));
+        ctx->stat_d2h_bytes += int64_t(out_rows[s]) * n * 4;
+      }
+      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
+      used[buf] = true;
+      buf ^= 1;
+    }
+    WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    return WB2_OK;
+  }();
+  cudaStreamSynchronize(ctx->stream);
+  cudaStreamSynchronize(ctx->copy_stream);
+  for (int i = 0; i < 2; ++i)
+    if (stage[i]) cudaFree(stage[i]);
+  if (t.base) cudaFree(t.base);
+  return rc;
 }
 
 }  // namespace wb2
@@ -424,110 +508,16 @@ int wb2_climatology_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime, 
   if (ncell == 0) return WB2_OK;
   WB2_REQUIRE(x != nullptr, "x is NULL");
   DeviceGuard guard(ctx->device);
-  const size_t esize = dtype == WB2_F32 ? 4 : 8;
-
-  // the time rows the selection touches; tables rebased to the first of them
-  int64_t t_lo = ntime, t_hi = -1;
-  const size_t n_items = size_t(nhour) * nday * nitem;
-  const size_t n_fill = p.fill ? size_t(nhour) * nitem : 0;
-  if (nres > 0) {
-    for (int64_t i = 0; i < nres; ++i)
-      if (res_count[i] > 0) {
-        t_lo = std::min(t_lo, res_start[i]);
-        t_hi = std::max(t_hi, res_start[i] + res_count[i] - 1);
-      }
-  } else {
-    for (size_t i = 0; i < n_items; ++i)
-      if (items[i] >= 0) t_lo = std::min(t_lo, items[i]), t_hi = std::max(t_hi, items[i]);
-    for (size_t i = 0; i < n_fill; ++i)
-      if (p.fill[i] >= 0) t_lo = std::min(t_lo, p.fill[i]), t_hi = std::max(t_hi, p.fill[i]);
-  }
-  const int64_t rows = t_hi >= t_lo ? t_hi - t_lo + 1 : 0;
-  if (rows == 0) t_lo = 0;
-  std::vector<int64_t> it_r(items, items + n_items), fill_r, start_r;
-  if (nres > 0) {
-    start_r.assign(res_start, res_start + nres);
-    for (auto& v : start_r) v -= t_lo;
-  } else {
-    for (auto& v : it_r)
-      if (v >= 0) v -= t_lo;
-  }
-  if (n_fill) {
-    fill_r.assign(p.fill, p.fill + n_fill);
-    if (nres == 0)
-      for (auto& v : fill_r)
-        if (v >= 0) v -= t_lo;
-  }
-
-  // band of cells: input rows + resampled days + outputs, double buffered
-  const int nstat = (mean_host ? 1 : 0) + (std_host ? 1 : 0);
-  const size_t out_rows = size_t(nhour) * nday_out;
-  const size_t per_cell = size_t(rows) * esize + size_t(nres) * 4 + nstat * out_rows * 4;
-  int64_t nb = static_cast<int64_t>(budget / (2 * per_cell));
-  nb = std::max<int64_t>(1, std::min(nb, ncell));
-  auto al = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_in = al(size_t(rows) * nb * esize), b_day = al(size_t(nres) * nb * 4);
-  const size_t b_out = al(out_rows * nb * 4);
-  const size_t stage_bytes = b_in + b_day + nstat * b_out;
-
-  ClimDeviceTables t;
-  char* stage[2] = {nullptr, nullptr};
-  const int rc = [&]() -> int {
-    WB2_TRY(clim_upload(ctx, p, it_r.data(), n_fill ? fill_r.data() : nullptr, &t));
-    for (int i = 0; i < 2; ++i)
-      WB2_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&stage[i]), stage_bytes));
-    const char* xh = static_cast<const char*>(x);
-    bool used[2] = {false, false};
-    int buf = 0;
-    for (int64_t c0 = 0; c0 < ncell; c0 += nb) {
-      const int64_t n = std::min(nb, ncell - c0);
-      char* in = stage[buf];
-      float* daily = reinterpret_cast<float*>(in + b_in);
-      float* om = reinterpret_cast<float*>(in + b_in + b_day);
-      float* os = om + (mean_host ? b_out / 4 : 0);
-      if (used[buf])
-        WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
-      if (rows > 0) {  // the band's whole selected series: one strided 2-D copy
-        WB2_CUDA_TRY(cudaMemcpy2DAsync(in, size_t(n) * esize,
-                                       xh + (size_t(t_lo) * ncell + c0) * esize,
-                                       size_t(ncell) * esize, size_t(n) * esize, size_t(rows),
-                                       cudaMemcpyHostToDevice, ctx->copy_stream));
-        ctx->stat_h2d_bytes += rows * n * int64_t(esize);
-      }
-      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
-      WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
-      const void* src = in;
-      if (nres > 0) {
-        WB2_TRY(clim_resample(ctx, reinterpret_cast<const float*>(in), n, n, p, start_r.data(),
-                              daily));
-        src = daily;
-      }
-      if (p.need_nan_fill)
-        WB2_CUDA_TRY(cudaMemsetAsync(om, 0xFF, nstat * b_out, ctx->stream));
-      WB2_TRY(clim_launch(ctx, src, dtype, n, n, t.args, mean_host ? om : nullptr,
-                          std_host ? os : nullptr));
-      float* dst[2] = {mean_host, std_host};
-      float* from[2] = {om, os};
-      for (int s = 0; s < 2; ++s) {
-        if (!dst[s]) continue;
-        WB2_CUDA_TRY(cudaMemcpy2DAsync(dst[s] + c0, size_t(ncell) * 4, from[s], size_t(n) * 4,
-                                       size_t(n) * 4, out_rows, cudaMemcpyDeviceToHost,
-                                       ctx->stream));
-        ctx->stat_d2h_bytes += int64_t(out_rows) * n * 4;
-      }
-      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
-      used[buf] = true;
-      buf ^= 1;
-    }
-    WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return WB2_OK;
-  }();
-  cudaStreamSynchronize(ctx->stream);
-  cudaStreamSynchronize(ctx->copy_stream);
-  for (int i = 0; i < 2; ++i)
-    if (stage[i]) cudaFree(stage[i]);
-  if (t.base) cudaFree(t.base);
-  return rc;
+  float* const out_host[2] = {mean_host ? mean_host : std_host, std_host};
+  const size_t rows = size_t(nhour) * nday_out;
+  const size_t out_rows[2] = {rows, rows};
+  const int nout = (mean_host ? 1 : 0) + (std_host ? 1 : 0);
+  return clim_stream_host(
+      ctx, x, dtype, ntime, ncell, p, budget, nout, out_host, out_rows,
+      [&](const void* src, int64_t n, const ClimArgs& tables, float* const* out) {
+        return clim_launch(ctx, src, dtype, n, n, tables, mean_host ? out[0] : nullptr,
+                           std_host ? out[nout - 1] : nullptr);
+      });
 }
 
 }  // extern "C"

@@ -1,4 +1,5 @@
-"""Day-of-year climatologies (mean and standard deviation) on the GPU.
+"""Day-of-year climatologies (mean, standard deviation, quantiles and SEEPS
+thresholds) on the GPU.
 
 Drop-in for the climatology functions of weatherbench2/utils.py and the
 computation of scripts/compute_climatology.py without Beam or zarr:
@@ -8,18 +9,33 @@ computation of scripts/compute_climatology.py without Beam or zarr:
   compute_daily_stat         utils.py:127-140
   compute_hourly_stat_fast   utils.py:217-272  (the `fast` method)
   compute_daily_stat_fast    utils.py:200-214, 275-287
+  Quantile, SEEPSThreshold   compute_climatology.py:130-177
   compute_climatology        compute_climatology.py:219-356 (`main`)
 
 The host turns the time selection into index tables (`_lib.ClimatologyPlan`):
 the reference's year stacking over the union of day-of-year labels
 (`xr.concat(dim='year')`, utils.py:97-103) or its `groupby('time.dayofyear')`.
-The CUDA kernel (csrc/climatology.cu) reads the (time, cells) series in place
-through them, accumulates float64 moments and applies the circular window.
+The CUDA kernels read the (time, cells) series in place through them:
+csrc/climatology.cu accumulates float64 moments and applies the circular
+window (mean, std); csrc/climatology_quantile.cu slides a sorted window over
+the day axis and takes xarray's weighted quantile of it (quantile, SEEPS).
 CUDA tensors stay on the device; NumPy arrays (np.memmap included) are streamed
 in bands of cells whose device footprint is bounded by `STREAM_BUDGET_BYTES`.
 
-Only the statistics 'mean' and 'std' are computed; the reference's 'seeps' and
-'quantile' climatologies are not (NotImplementedError).
+The quantile and SEEPS statistics exist for the `explicit` method only; the
+`fast` functions refuse them, as the reference does.  `Quantile(qs).compute`
+and `SEEPSThreshold(mm, var).compute` are accepted as `stat_fn` by
+compute_hourly_stat / compute_daily_stat, which is how the reference script
+passes them; calling `.compute` directly on other dimensions is not supported
+(NotImplementedError).  At most 16 quantiles per call, and at most 8192
+samples (stacked years x window_size) per window (ValueError).
+
+Two deviations from the reference's compute_climatology: 'quantile' without
+`quantiles=` raises NotImplementedError (the reference: ValueError), and
+'seeps' without `seeps_dry_threshold_mm=` raises NotImplementedError instead
+of defaulting to {'total_precipitation_24hr': 0.25,
+'total_precipitation_6hr': 0.1}.  Statistics other than mean, std, quantile
+and seeps are not computed (NotImplementedError).
 """
 from __future__ import annotations
 
@@ -57,13 +73,75 @@ def _check_window(window_size: int):
                      'the triangular weights of a 1-day window are 0 / 0')
 
 
-def _check_stat(stat_fn: StatFn):
-  if isinstance(stat_fn, str) and stat_fn in ('mean', 'std'):
+def _check_stat(stat_fn: StatFn, quantiles=None, seeps_dry_threshold_mm=None):
+  if isinstance(stat_fn, str) and (
+      stat_fn in ('mean', 'std') or
+      (stat_fn == 'quantile' and quantiles is not None) or
+      (stat_fn == 'seeps' and seeps_dry_threshold_mm is not None)):
     return
+  hint = {'quantile': ' (pass quantiles=[...])',
+          'seeps': ' (pass seeps_dry_threshold_mm={variable: mm})'}
   raise NotImplementedError(
       f'stat {stat_fn!r} not implemented: the GPU climatology computes the '
-      "statistics 'mean' and 'std'; the 'seeps' and 'quantile' statistics are "
+      "statistics 'mean' and 'std' (both methods), 'quantile' given quantiles= "
+      "and 'seeps' given seeps_dry_threshold_mm= (explicit method); anything "
+      'else is out of its scope' + hint.get(stat_fn, '')
+      if isinstance(stat_fn, str) else
+      f'stat {stat_fn!r} not implemented: only the explicit functions take '
+      'Quantile(...).compute / SEEPSThreshold(...).compute; anything else is '
       'out of its scope')
+
+
+class Quantile:
+  """Weighted quantiles over (window, year) (compute_climatology.py:130-144).
+  `stat_fn=Quantile(qs).compute` carries the quantiles into the GPU path."""
+
+  def __init__(self, quantiles: Sequence[float]):
+    self.quantiles = quantiles
+
+  def compute(self, ds, dim, weights=None):
+    raise NotImplementedError(
+        'Quantile.compute runs inside compute_hourly_stat / compute_daily_stat '
+        '(stat_fn=Quantile(qs).compute); other dimensions are out of its scope')
+
+
+class SEEPSThreshold:
+  """SEEPS heavy-precipitation threshold (the weighted 2/3 quantile of the wet
+  samples) and dry fraction (compute_climatology.py:147-177).
+  `stat_fn=SEEPSThreshold(mm, var).compute` carries them into the GPU path."""
+
+  def __init__(self, dry_threshold_mm: float, var: str):
+    self.dry_threshold_m = dry_threshold_mm / 1000.0
+    self.var = var
+
+  def compute(self, ds, dim, weights=None):
+    raise NotImplementedError(
+        'SEEPSThreshold.compute runs inside compute_hourly_stat / '
+        'compute_daily_stat (stat_fn=SEEPSThreshold(mm, var).compute); other '
+        'dimensions are out of its scope')
+
+
+def _quantile_spec(stat_fn):
+  """The Quantile / SEEPSThreshold a stat_fn carries, or None."""
+  if isinstance(stat_fn, (Quantile, SEEPSThreshold)):
+    return stat_fn
+  owner = getattr(stat_fn, '__self__', None)
+  if isinstance(owner, (Quantile, SEEPSThreshold)) and getattr(
+      stat_fn, '__func__', None) is type(owner).compute:
+    return owner
+  return None
+
+
+def _quantile_values(quantiles) -> np.ndarray:
+  q = np.atleast_1d(np.asarray(quantiles, dtype=np.float64))
+  if q.ndim != 1 or not q.size:
+    raise ValueError(f'quantiles must be a non-empty sequence, got {quantiles!r}')
+  if not np.all((q >= 0) & (q <= 1)):
+    raise ValueError(f'Quantiles must be in the range [0, 1], got {quantiles!r}')
+  if q.size > _lib.CLIM_MAX_QUANTILES:
+    raise ValueError(f'at most {_lib.CLIM_MAX_QUANTILES} quantiles per call '
+                     f'(got {q.size})')
+  return q
 
 
 # -- index tables -------------------------------------------------------------
@@ -157,6 +235,32 @@ def _plan(times, clim_years, hours: Optional[Sequence[int]], method: int,
 
 
 # -- execution ------------------------------------------------------------------
+def _series(da: xl.DataArray, plan):
+  """(x, dtype code, other dims, their shape, ncell, ntime, on device): the
+  (time, cells) series the kernels read, float64 kept unless resampled."""
+  ti = da.dims.index('time')
+  other = tuple(d for d in da.dims if d != 'time')
+  oshape = tuple(da.sizes[d] for d in other)
+  ncell = int(np.prod(oshape)) if oshape else 1
+  ntime = da.sizes['time']
+  data = da.data
+  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
+    import torch  # pylint: disable=import-outside-toplevel
+    x = data.movedim(ti, 0)
+    if x.dtype != torch.float64 or plan.nres:
+      x = x.to(torch.float32)
+    x = x.contiguous()
+    code = _lib.F64 if x.dtype == torch.float64 else _lib.F32
+    return x, code, other, oshape, ncell, ntime, True
+  x = np.asarray(data)
+  if ti:
+    x = np.moveaxis(x, ti, 0)
+  dt = np.float64 if x.dtype == np.float64 and not plan.nres else np.float32
+  x = np.ascontiguousarray(x, dtype=dt)
+  code = _lib.F64 if dt == np.float64 else _lib.F32
+  return x, code, other, oshape, ncell, ntime, False
+
+
 def _run(ds: xl.Dataset, plan, labels, hours, stats: Sequence[str]) -> dict:
   """{stat: {variable: DataArray}} for every variable with a time axis."""
   ctx = _lib.default_context()
@@ -164,38 +268,21 @@ def _run(ds: xl.Dataset, plan, labels, hours, stats: Sequence[str]) -> dict:
   for name, da in ds.items():
     if 'time' not in da.dims:
       continue
-    ti = da.dims.index('time')
-    other = tuple(d for d in da.dims if d != 'time')
-    oshape = tuple(da.sizes[d] for d in other)
-    ncell = int(np.prod(oshape)) if oshape else 1
-    ntime = da.sizes['time']
+    x, code, other, oshape, ncell, ntime, device = _series(da, plan)
     nrow = (plan.nhour, plan.nday_out)
-    data = da.data
-    if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
+    if device:
       import torch  # pylint: disable=import-outside-toplevel
-      x = data.movedim(ti, 0)
-      if x.dtype != torch.float64 or plan.nres:
-        x = x.to(torch.float32)
-      x = x.contiguous()
       res = {s: torch.empty(nrow + oshape, device=x.device,
                             dtype=torch.float32) for s in stats}
       ptr = {s: res[s].data_ptr() if s in res else None for s in ('mean', 'std')}
-      ctx.climatology(x.data_ptr(),
-                      _lib.F64 if x.dtype == torch.float64 else _lib.F32,
-                      ntime, ncell, plan, ptr['mean'], ptr['std'])
+      ctx.climatology(x.data_ptr(), code, ntime, ncell, plan, ptr['mean'],
+                      ptr['std'])
     else:
-      x = np.asarray(data)
-      if ti:
-        x = np.moveaxis(x, ti, 0)
-      dt = np.float64 if x.dtype == np.float64 and not plan.nres else np.float32
-      x = np.ascontiguousarray(x, dtype=dt)
       res = {s: ctx.pinned_result(nrow + oshape, np.float32) for s in stats}
       ptr = {s: res[s].ctypes.data if s in res else None
              for s in ('mean', 'std')}
-      ctx.climatology_host(x.ctypes.data,
-                           _lib.F64 if dt == np.float64 else _lib.F32, ntime,
-                           ncell, plan, STREAM_BUDGET_BYTES, ptr['mean'],
-                           ptr['std'])
+      ctx.climatology_host(x.ctypes.data, code, ntime, ncell, plan,
+                           STREAM_BUDGET_BYTES, ptr['mean'], ptr['std'])
     coords = {k: c for k, c in da.coords.items() if 'time' not in c.dims}
     coords['dayofyear'] = xl.Coord(('dayofyear',), labels)
     if hours is None:
@@ -231,6 +318,79 @@ def _compute(obs, window_size: int, clim_years: slice,
   return out
 
 
+def _run_quantile(ds: xl.Dataset, plan, labels, hours, spec) -> dict:
+  """{name: DataArray}: the quantiles of every variable with a time axis
+  (names kept), or the SEEPS pair of `spec.var`."""
+  ctx = _lib.default_context()
+  seeps = isinstance(spec, SEEPSThreshold)
+  qs = np.array([2 / 3]) if seeps else _quantile_values(spec.quantiles)
+  thr = spec.dry_threshold_m if seeps else None
+  names = [spec.var] if seeps else [n for n, da in ds.items()
+                                    if 'time' in da.dims]
+  lead = ('dayofyear',) if hours is None else ('hour', 'dayofyear')
+  out = {}
+  for name in names:
+    da = ds[name]
+    x, code, other, oshape, ncell, ntime, device = _series(da, plan)
+    qshape = (plan.nhour, qs.size, plan.nday_out) + oshape
+    dshape = (plan.nhour, plan.nday_out) + oshape
+    if device:
+      import torch  # pylint: disable=import-outside-toplevel
+      res = torch.empty(qshape, device=x.device, dtype=torch.float32)
+      dry = (torch.empty(dshape, device=x.device, dtype=torch.float32)
+             if seeps else None)
+      ctx.climatology_quantile(x.data_ptr(), code, ntime, ncell, plan, qs, thr,
+                               res.data_ptr(),
+                               dry.data_ptr() if seeps else None)
+    else:
+      res = ctx.pinned_result(qshape, np.float32)
+      dry = ctx.pinned_result(dshape, np.float32) if seeps else None
+      ctx.climatology_quantile_host(x.ctypes.data, code, ntime, ncell, plan, qs,
+                                    thr, STREAM_BUDGET_BYTES, res.ctypes.data,
+                                    dry.ctypes.data if seeps else None)
+    coords = {k: c for k, c in da.coords.items() if 'time' not in c.dims}
+    coords['dayofyear'] = xl.Coord(('dayofyear',), labels)
+    if hours is not None:
+      coords['hour'] = xl.Coord(('hour',), np.asarray(hours))
+    dims = lead + other
+    shape = dshape[1:] if hours is None else dshape
+    if seeps:
+      for key, v in ((f'{name}_seeps_threshold', res.reshape(shape)),
+                     (f'{name}_seeps_dry_fraction', dry.reshape(shape))):
+        out[key] = xl.DataArray(v, dims, coords, key, da.attrs)
+    else:
+      coords['quantile'] = xl.Coord(('quantile',), qs)
+      if hours is None:
+        dims = ('quantile',) + dims
+        v = res.reshape(qshape[1:])
+      else:
+        dims = ('hour', 'quantile') + dims[1:]
+        v = res
+      out[name] = xl.DataArray(v, dims, coords, name, da.attrs)
+  return out
+
+
+def _compute_quantile(obs, window_size: int, clim_years: slice,
+                      hours: Optional[Sequence[int]], spec) -> xl.Dataset:
+  """The Quantile / SEEPSThreshold climatology, explicit method; the daily
+  statistics take the daily resample (utils.py:127-140)."""
+  _check_window(window_size)
+  if not isinstance(spec, SEEPSThreshold):
+    _quantile_values(spec.quantiles)
+  ds = xl.from_xarray(obs)
+  if isinstance(spec, SEEPSThreshold) and spec.var not in ds:
+    raise KeyError(spec.var)
+  plan, labels = _plan(ds.coords['time'].values, clim_years, hours, EXPLICIT,
+                       hours is None, window_size)
+  if plan.nitem * window_size > _lib.CLIM_QUANTILE_MAX_SAMPLES:
+    raise ValueError(
+        f'{plan.nitem} stacked years x window_size {window_size} exceeds the '
+        f'{_lib.CLIM_QUANTILE_MAX_SAMPLES} samples per window of the GPU '
+        'quantile climatology')
+  return xl.Dataset(_run_quantile(ds, plan, labels, hours, spec),
+                    attrs=ds.attrs)
+
+
 def _public(obs, result: xl.Dataset):
   return xl.to_xarray(result) if xl.is_native_xarray(obs) else result
 
@@ -242,6 +402,10 @@ def _hours(hour_interval: int):
 def compute_hourly_stat(obs, window_size: int, clim_years: slice,
                         hour_interval: int, stat_fn: StatFn = 'mean'):
   """Climatology by hour of day and day of year, `explicit` method."""
+  spec = _quantile_spec(stat_fn)
+  if spec is not None:
+    return _public(obs, _compute_quantile(obs, window_size, clim_years,
+                                          _hours(hour_interval), spec))
   _check_stat(stat_fn)
   res = _compute(obs, window_size, clim_years, _hours(hour_interval), EXPLICIT,
                  [stat_fn])
@@ -251,6 +415,10 @@ def compute_hourly_stat(obs, window_size: int, clim_years: slice,
 def compute_daily_stat(obs, window_size: int, clim_years: slice,
                        stat_fn: StatFn = 'mean'):
   """Climatology by day of year of the daily means, `explicit` method."""
+  spec = _quantile_spec(stat_fn)
+  if spec is not None:
+    return _public(obs, _compute_quantile(obs, window_size, clim_years, None,
+                                          spec))
   _check_stat(stat_fn)
   res = _compute(obs, window_size, clim_years, None, EXPLICIT, [stat_fn])
   return _public(obs, res[stat_fn])
@@ -277,30 +445,58 @@ def compute_climatology(obs, *, frequency: str = 'hourly',
                         hour_interval: int = 1, window_size: int = 61,
                         start_year: int = 1990, end_year: int = 2020,
                         statistics: Sequence[str] = ('mean',),
-                        method: str = 'explicit'):
+                        method: str = 'explicit',
+                        quantiles: Optional[Sequence[float]] = None,
+                        seeps_dry_threshold_mm: Optional[dict] = None):
   """scripts/compute_climatology.py without Beam or zarr: variables without a
   time axis are dropped, time is selected over [start_year, end_year] (both
-  inclusive), the mean keeps the variable's name and the std is `<var>_std`.
+  inclusive), the mean keeps the variable's name, the std is `<var>_std` and
+  the quantiles `<var>_quantile` (dims hour, quantile, dayofyear, ...).  SEEPS
+  gives `<var>_seeps_threshold` and `<var>_seeps_dry_fraction` for the
+  variables of `seeps_dry_threshold_mm` ({variable: dry threshold in mm}).
   Dims (hour, dayofyear, ...) for hourly, (dayofyear, ...) for daily; the day
   axis holds the day-of-year labels present in the selection.  Mean and std
   are computed from one read of the data."""
   stats = [statistics] if isinstance(statistics, str) else list(statistics)
   for s in stats:
-    _check_stat(s)
+    _check_stat(s, quantiles, seeps_dry_threshold_mm)
   if frequency not in ('hourly', 'daily'):
     raise NotImplementedError(f'Frequency {frequency} not implemented.')
   if method not in ('explicit', 'fast'):
     raise NotImplementedError(
         f'method {method} for climatological frequency {frequency} not '
         'implemented.')
+  if method != 'explicit':
+    if 'seeps' in stats:
+      raise NotImplementedError('SEEPS only tested for explicit.')
+    if 'quantile' in stats:
+      raise NotImplementedError(f'stat {Quantile(quantiles).compute} not '
+                                'implemented.')
+  if 'quantile' in stats:
+    _quantile_values(quantiles)
   hours = _hours(hour_interval) if frequency == 'hourly' else None
-  res = _compute(obs, window_size, slice(str(start_year), str(end_year)),
-                 hours, EXPLICIT if method == 'explicit' else FAST, stats)
+  years = slice(str(start_year), str(end_year))
+  moments = [s for s in stats if s in ('mean', 'std')]
+  res = (_compute(obs, window_size, years, hours,
+                  EXPLICIT if method == 'explicit' else FAST, moments)
+         if moments else {})
   ds = xl.from_xarray(obs)
   out = xl.Dataset(attrs=ds.attrs)
   for s in stats:
-    for name, da in res[s].items():
-      key = name if s == 'mean' else f'{name}_{s}'
-      da.name = key
-      out[key] = da
+    if s == 'quantile':
+      q = _compute_quantile(obs, window_size, years, hours,
+                            Quantile(quantiles))
+      for name, da in q.items():
+        da.name = f'{name}_quantile'
+        out[da.name] = da
+    elif s == 'seeps':
+      for var, mm in seeps_dry_threshold_mm.items():
+        for name, da in _compute_quantile(obs, window_size, years, hours,
+                                          SEEPSThreshold(mm, var)).items():
+          out[name] = da
+    else:
+      for name, da in res[s].items():
+        key = name if s == 'mean' else f'{name}_{s}'
+        da.name = key
+        out[key] = da
   return _public(obs, out)
