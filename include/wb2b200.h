@@ -322,15 +322,17 @@ int wb2_spectrum_interp(wb2_ctx* ctx, const float* spec, int64_t nfield,
  *              ignored; utils.py:105)
  *   hour_nday  host [nhour]: day slots of hour h, the period of the circular
  *              window (the window wraps positionally over slots 0..n-1)
- *   out_row    host [nhour][nday]: output row of each slot, < nday_out; rows an
- *              hour does not produce are NaN
+ *   out_row    host [nhour][nday]: output row of each slot, < nday_out, distinct
+ *              within an hour (a repeated row is an error); rows an hour does
+ *              not produce are NaN
  *   method     0 explicit: xarray's weighted mean / population std over (window,
  *              year) with the triangular weights of create_window_weights
  *              1 fast: per-slot mean / std (ddof 0), then the mean over the
  *              window of weight * value, NaN skipped (count denominator)
  *   mean, std  device [nhour][nday_out][ncell] float32; either may be NULL
- * Moments accumulate in float64 around a per-cell shift; one read of x serves
- * both statistics.  window_size: odd, >= 3.                                      */
+ * Moments accumulate in float64 around a per-cell shift (a finite value of the
+ * cell among up to 512 table entries spread over the hour's table, the fill
+ * applied); one read of x serves both statistics.  window_size: odd, >= 3.      */
 int wb2_climatology(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime,
                     int64_t ncell, int64_t nres, const int64_t* res_start,
                     const int32_t* res_count, int32_t nhour, int32_t nday,
@@ -369,8 +371,10 @@ int wb2_climatology_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime,
  *              1: samples x < dry_threshold (compared in the series' precision)
  *                 are dropped like NaN before the quantiles, and dry_fraction =
  *                 the unweighted mean of (x < dry_threshold) over all
- *                 nyear * window_size samples (NaN is not dry); SEEPSThreshold
- *                 is nquantile 1, quantiles {2/3}
+ *                 nyear * window_size samples (NaN is not dry; nyear of hour h
+ *                 = the item columns with a step in some slot of the hour, so
+ *                 an hour without any is NaN); SEEPSThreshold is nquantile 1,
+ *                 quantiles {2/3}
  *   out        device [nhour][nquantile][nday_out][ncell] float32
  *   dry_fraction  device [nhour][nday_out][ncell] float32 (seeps 1)
  * nitem * window_size <= 8192.                                                   */

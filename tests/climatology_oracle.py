@@ -73,20 +73,26 @@ def rolling_stat(times, x, window_size, stat):
   pad = [(0, 0), (half, half)] + [(0, 0)] * (x.ndim - 1)
   padded = np.pad(stacked, pad, mode='wrap')
   out = np.full((labels.size,) + x.shape[1:], np.nan)
-  wb = w.reshape((1, -1) + (1,) * (x.ndim - 1))
   for d in range(labels.size):
-    win = padded[:, d:d + window_size]  # (year, window, ...)
-    ok = ~np.isnan(win)
-    sw = (wb * ok).sum(axis=(0, 1))
-    with np.errstate(invalid='ignore', divide='ignore'):
-      mean = np.where(ok, wb * win, 0.0).sum(axis=(0, 1)) / sw
-      if stat == 'mean':
-        res = mean
-      else:
-        dev = np.where(ok, wb * (win - mean) ** 2, 0.0).sum(axis=(0, 1))
-        res = np.sqrt(dev / sw)
-    out[d] = np.where(sw == 0, np.nan, res)
+    out[d] = weighted_stat(padded[:, d:d + window_size], w, stat)
   return labels, out
+
+
+def weighted_stat(win, w, stat):
+  """xarray's weighted mean / population std of one window win (year, window,
+  ...) over (year, window) with the tap weights w [window], NaN skipped; NaN
+  where the weight sum is 0."""
+  wb = np.asarray(w, np.float64).reshape((1, -1) + (1,) * (win.ndim - 2))
+  ok = ~np.isnan(win)
+  sw = (wb * ok).sum(axis=(0, 1))
+  with np.errstate(invalid='ignore', divide='ignore'):
+    mean = np.where(ok, wb * win, 0.0).sum(axis=(0, 1)) / sw
+    if stat == 'mean':
+      res = mean
+    else:
+      dev = np.where(ok, wb * (win - mean) ** 2, 0.0).sum(axis=(0, 1))
+      res = np.sqrt(dev / sw)
+  return np.where(sw == 0, np.nan, res)
 
 
 def dayofyear_stat(times, x, stat):

@@ -12,10 +12,12 @@
 // One CTA owns 8 cells (one 32-B sector of float32 per time step) and the whole
 // day axis of one hour:
 //   phase 1  per (day slot, cell) the float64 moments over the slot's items:
-//            count, sum (x - K), sum (x - K)^2, K = a per-cell shift (the
-//            first finite value of the cell) so that fields with a large mean
-//            keep their variance.  The explicit method fills a NaN / missing
-//            item of year y with year y's day-365 value on load
+//            count, sum (x - K), sum (x - K)^2, K = a per-cell shift (a
+//            finite value of the cell, found by probing up to 512 table
+//            entries spread over the whole table) so that fields with a
+//            large mean keep their variance, even when the first entries of
+//            the table are missing or NaN.  The explicit method fills a NaN /
+//            missing item of year y with year y's day-365 value on load
 //            (utils.py:105).  The moments live in shared memory (20 B per day
 //            and cell: 58.5 KB for 366 days), never in HBM.
 //   phase 2  the circular 2h+1-tap triangular window over the positional day
@@ -44,6 +46,7 @@ constexpr int kClimCells = 8;   // cells per CTA
 constexpr int kClimLanes = 32;  // day lanes per CTA
 constexpr int kClimThreads = kClimCells * kClimLanes;
 constexpr int kClimMaxDays = 1400;  // shared memory: 160 B per day slot
+constexpr int kClimShiftSamples = 512;  // table entries probed for the shift
 
 __device__ __forceinline__ int wrap_day(int i, int n) {
   i %= n;
@@ -55,6 +58,7 @@ __global__ void __launch_bounds__(kClimThreads) climatology_kernel(const T* __re
                                                                    ClimArgs a) {
   extern __shared__ double clim_smem[];
   __shared__ double shift[kClimCells];
+  __shared__ int first[kClimCells];
   double* s1 = clim_smem;                 // [nday][8]
   double* s2 = s1 + a.nday * kClimCells;  // [nday][8]
   float* cnt = reinterpret_cast<float*>(s2 + a.nday * kClimCells);
@@ -68,20 +72,45 @@ __global__ void __launch_bounds__(kClimThreads) climatology_kernel(const T* __re
   const int64_t* fill = a.fill ? a.fill + int64_t(h) * nitem : nullptr;
   const T* xc = x + (live ? cell : 0);
 
-  if (dl == 0) {  // the shift K: first finite value among the first items
-    double k = 0.0;
-    const int lim = min(n * nitem, 256);
-    for (int q = 0; live && q < lim; ++q) {
-      const int64_t t = items[q];
-      if (t < 0) continue;
-      const double v = double(ldg_stream(xc + t * a.tstride));
+  // The shift K: the cell's value at the first of kClimShiftSamples table
+  // entries, spread evenly over the hour's whole table (every entry when it
+  // has fewer), that is finite after the fill.  Day lane 0 probes entry 0,
+  // which settles almost every cell with one load; otherwise the 32 day lanes
+  // of the cell probe in parallel, so a cell that is NaN everywhere costs
+  // each lane kClimShiftSamples / 32 probes.  K = 0 only when no probe is
+  // finite.
+  const int64_t nentry = int64_t(n) * nitem;
+  const int nprobe = nentry < kClimShiftSamples ? int(nentry) : kClimShiftSamples;
+  auto probe = [&](int i) {  // the value at entry i of the nprobe, fill applied
+    const int64_t q = nprobe == nentry ? i : int64_t(i) * nentry / nprobe;
+    const int64_t t = items[q];
+    double v = t >= 0 ? double(ldg_stream(xc + t * a.tstride)) : CUDART_NAN;
+    if (fill != nullptr && !(v == v)) {
+      const int64_t f = fill[q % nitem];
+      v = f >= 0 ? double(ldg_stream(xc + f * a.tstride)) : CUDART_NAN;
+    }
+    return v;
+  };
+  if (dl == 0) {
+    const double v = live ? probe(0) : CUDART_NAN;
+    shift[cl] = v == v ? v : 0.0;
+    first[cl] = v == v ? 0 : kClimShiftSamples;
+  }
+  __syncthreads();
+  int hit = kClimShiftSamples;
+  double hv = 0.0;
+  if (first[cl] != 0)
+    for (int i = dl; live && i < nprobe; i += kClimLanes) {
+      const double v = probe(i);
       if (v == v) {
-        k = v;
+        hit = i;
+        hv = v;
+        atomicMin(&first[cl], i);
         break;
       }
     }
-    shift[cl] = k;
-  }
+  __syncthreads();
+  if (hit < kClimShiftSamples && hit == first[cl]) shift[cl] = hv;  // one lane
   __syncthreads();
   const double k = shift[cl];
 
@@ -209,6 +238,7 @@ int clim_validate(int64_t ntime, int64_t nres, const int64_t* res_start,
                   "res_start[%lld] out of range", static_cast<long long>(i));
   }
   p->need_nan_fill = false;
+  std::vector<int32_t> row_owner(size_t(nday_out), -1);  // hour that wrote the row
   for (int32_t h = 0; h < nhour; ++h) {
     const int32_t n = hour_nday[h];
     WB2_REQUIRE(n >= 1 && n <= nday, "hour_nday[%d] = %d out of 1..%d", h, n, nday);
@@ -216,6 +246,10 @@ int clim_validate(int64_t ntime, int64_t nres, const int64_t* res_start,
     for (int32_t d = 0; d < n; ++d) {
       const int32_t r = out_row[int64_t(h) * nday + d];
       WB2_REQUIRE(r >= 0 && r < nday_out, "out_row[%d][%d] = %d out of range", h, d, r);
+      WB2_REQUIRE(row_owner[size_t(r)] != h,
+                  "out_row[%d][%d] = %d repeats a row of hour %d (rows must be distinct)",
+                  h, d, r, h);
+      row_owner[size_t(r)] = h;
       for (int32_t j = 0; j < nitem; ++j) {
         const int64_t t = items[(int64_t(h) * nday + d) * nitem + j];
         WB2_REQUIRE(t >= -1 && t < nsrc, "items[%d][%d][%d] = %lld out of range", h, d, j,
@@ -457,7 +491,7 @@ int wb2_climatology(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime, int64
   WB2_NVTX("wb2_climatology");
   WB2_REQUIRE(ctx != nullptr, "ctx is NULL");
   WB2_REQUIRE(dtype == WB2_F32 || dtype == WB2_F64, "dtype must be WB2_F32 or WB2_F64");
-  WB2_REQUIRE(nres == 0 || dtype == WB2_F32, "the daily resample takes float32 input");
+  WB2_REQUIRE(nres == 0 || dtype == WB2_F32, "nres > 0 (the daily resample) takes float32 input");
   WB2_REQUIRE(ncell >= 0, "ncell < 0");
   WB2_REQUIRE(mean || std, "neither mean nor std requested");
   ClimPlan p;
@@ -499,7 +533,7 @@ int wb2_climatology_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime, 
   WB2_NVTX("wb2_climatology_host");
   WB2_REQUIRE(ctx != nullptr, "ctx is NULL");
   WB2_REQUIRE(dtype == WB2_F32 || dtype == WB2_F64, "dtype must be WB2_F32 or WB2_F64");
-  WB2_REQUIRE(nres == 0 || dtype == WB2_F32, "the daily resample takes float32 input");
+  WB2_REQUIRE(nres == 0 || dtype == WB2_F32, "nres > 0 (the daily resample) takes float32 input");
   WB2_REQUIRE(ncell >= 0, "ncell < 0");
   WB2_REQUIRE(mean_host || std_host, "neither mean nor std requested");
   ClimPlan p;

@@ -342,7 +342,7 @@ static int quant_prepare(wb2_ctx* ctx, int dtype, int64_t ncell, int64_t nres, i
                          const double* quantiles, int32_t seeps, double dry_threshold,
                          const float* dry_fraction, QuantArgs* q, double** block_dev) {
   WB2_REQUIRE(dtype == WB2_F32 || dtype == WB2_F64, "dtype must be WB2_F32 or WB2_F64");
-  WB2_REQUIRE(nres == 0 || dtype == WB2_F32, "the daily resample takes float32 input");
+  WB2_REQUIRE(nres == 0 || dtype == WB2_F32, "nres > 0 (the daily resample) takes float32 input");
   WB2_REQUIRE(ncell >= 0, "ncell < 0");
   WB2_REQUIRE(nq >= 1 && nq <= kQuantMaxQ, "nquantile must be in 1..%d (got %d)", kQuantMaxQ,
               nq);
