@@ -11,6 +11,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel spectrum # K4, configs[4]
   python benchmarks/bench_kernels.py --kernel climatology --steps 3
   python benchmarks/bench_kernels.py --kernel climatology_quantile --steps 2
+  python benchmarks/bench_kernels.py --kernel resample --steps 5
 """
 import argparse
 import json
@@ -494,12 +495,97 @@ def bench_climatology_quantile(args):
         flush=True)
 
 
+def resample_bytes(nouter, ntime, ninner, nout, nstat, esize=4, window=0,
+                   block=256):
+  """Bytes a time resample / rolling window needs: the input read once (plus,
+  rolling, the w-1 halo rows each block of `block` outputs stages again) and
+  every output written once."""
+  halo = (window - 1) * -(-ntime // block) if window else 0
+  return (nouter * (ntime + halo) * ninner + nstat * nouter * nout * ninner
+          ) * esize
+
+
+def bench_resample(args):
+  """Device-resident 721 x 1440, 6-hourly for 2 years (12.1 GB): daily mean +
+  min + max (resample 1D) and a rolling 7-day mean (28 steps); then a
+  13 x 121 x 240 series, 6-hourly for 5 years, streamed from host memory:
+  weekly mean."""
+  import time
+  import numpy as np
+  import pandas as pd
+  torch, _lib, ctx = setup()
+  from weatherbench2_b200 import resampling
+  card = _card()
+  times = np.arange(np.datetime64('2019-01-01', 'ns'),
+                    np.datetime64('2021-01-01', 'ns'), np.timedelta64(6, 'h'))
+  ncell = NLAT * NLON
+  x = torch.empty((times.size, ncell), device='cuda', dtype=torch.float32)
+  gen = torch.Generator(device='cuda').manual_seed(0)
+  for i in range(0, times.size, 512):
+    x[i:i + 512].normal_(generator=gen)
+  _, start, count = resampling._bins(times, pd.Timedelta('1D'), 'left')  # pylint: disable=protected-access
+  out = [torch.empty((count.size, ncell), device='cuda') for _ in range(3)]
+  fn = lambda: ctx.time_window_stats(
+      x.data_ptr(), _lib.F32, 1, times.size, ncell, start, count, 0, False,
+      out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(), None)
+  ms = timeit(fn, args.steps, warmup=2)
+  nbytes = resample_bytes(1, times.size, ncell, count.size, 3)
+  report('resample device 721x1440 6-hourly 2y daily mean+min+max', ms,
+         nbytes, times.size * ncell, 'values',
+         dict(card, input_GB=times.size * ncell * 4 / 1e9))
+  del out
+  roll = torch.empty_like(x)
+  fn = lambda: ctx.time_window_stats(
+      x.data_ptr(), _lib.F32, 1, times.size, ncell, None, None, 28, False,
+      roll.data_ptr(), None, None, None)
+  ms = timeit(fn, args.steps, warmup=2)
+  nbytes = resample_bytes(1, times.size, ncell, times.size, 1, window=28)
+  report('resample device 721x1440 6-hourly 2y rolling 7-day mean (w=28)', ms,
+         nbytes, times.size * ncell, 'values', dict(card))
+  del x, roll
+  torch.cuda.empty_cache()
+  # streamed from host memory: (time, level, lat, lon), weekly mean
+  times = np.arange(np.datetime64('2016-01-01', 'ns'),
+                    np.datetime64('2021-01-01', 'ns'), np.timedelta64(6, 'h'))
+  ncell = 13 * 121 * 240
+  block = np.random.default_rng(0).standard_normal((61, ncell),
+                                                   dtype=np.float32)
+  xh = np.empty((times.size, ncell), np.float32)
+  for i in range(0, times.size, 61):
+    xh[i:i + 61] = block[:times.size - i]
+  _, start, count = resampling._bins(times, pd.Timedelta('7D'), 'left')  # pylint: disable=protected-access
+  mh = np.empty((count.size, ncell), np.float32)
+  run = lambda: ctx.time_window_stats_host(
+      xh.ctypes.data, _lib.F32, 1, times.size, ncell, start, count, 0, False,
+      resampling.STREAM_BUDGET_BYTES, mh.ctypes.data, None, None, None)
+  run()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    run()
+  s = (time.perf_counter() - t0) / args.steps
+  probe = xh.reshape(-1)[:1 << 28]  # the pageable host -> device rate, 1 GiB
+  dev = torch.empty(probe.size, device='cuda', dtype=torch.float32)
+  dev.copy_(torch.from_numpy(probe))
+  torch.cuda.synchronize()
+  t0 = time.perf_counter()
+  for _ in range(3):
+    dev.copy_(torch.from_numpy(probe))
+  torch.cuda.synchronize()
+  h2d = 3 * probe.nbytes / (time.perf_counter() - t0) / 1e9
+  nbytes = resample_bytes(1, times.size, ncell, count.size, 1)
+  gbs = nbytes / s / 1e9
+  print(json.dumps(dict(
+      card, kernel='resample streamed 13x121x240 6-hourly 5y weekly mean',
+      ms=s * 1e3, algorithmic_GB=nbytes / 1e9, achieved_GBps=gbs,
+      h2d_pageable_GBps=h2d, frac_of_h2d=gbs / h2d)), flush=True)
+
+
 if __name__ == '__main__':
   ap = argparse.ArgumentParser()
   ap.add_argument('--kernel', required=True,
                   choices=['ens', 'energy', 'det', 'regrid', 'spectrum',
                            'maps', 'threshold', 'climatology',
-                           'climatology_quantile'])
+                           'climatology_quantile', 'resample'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -508,4 +594,5 @@ if __name__ == '__main__':
    'spectrum': bench_spectrum, 'maps': bench_maps,
    'threshold': bench_threshold,
    'climatology': bench_climatology,
-   'climatology_quantile': bench_climatology_quantile}[a.kernel](a)
+   'climatology_quantile': bench_climatology_quantile,
+   'resample': bench_resample}[a.kernel](a)

@@ -399,6 +399,49 @@ int wb2_climatology_quantile_host(wb2_ctx* ctx, const void* x, int dtype, int64_
                                   double dry_threshold, size_t budget, float* out,
                                   float* dry_fraction);
 
+/* ---- time resampling and rolling windows ------------------------------------------
+ * wb2_time_window_stats replaces xarray's resample(...).mean/min/max/sum and
+ * rolling(..., min_periods=None).mean/min/max/sum along one axis, the computation
+ * of scripts/resample_in_time.py.  x is [nouter][ntime][ninner] (float32 or
+ * float64, read in place: a forecast resampled along prediction_timedelta has
+ * outer = time, inner = the cells after it).  Exactly one of:
+ *   bins      resample: bin_start / bin_count host [nbin]; output b reduces the
+ *             bin_count[b] steps from bin_start[b].  Bins are in order and
+ *             disjoint (bin_start[b] >= bin_start[b-1] + bin_count[b-1]),
+ *             bin_count >= 0, and lie inside [0, ntime) (an empty bin's start is
+ *             at most ntime).  window must be 0.
+ *   window    rolling, > 0: output t reduces steps [t - window + 1, t]; nbin must
+ *             be 0 and the bin arrays NULL.  There are ntime outputs.
+ * Per output (mean / min / max / sum):
+ *   resample, skipna 0   any NaN in the bin -> NaN
+ *   resample, skipna 1   NaN skipped; an all-NaN bin gives NaN, except sum = 0
+ *   empty bin            NaN for every statistic, sum included
+ *   rolling              NaN when t < window - 1 or when any value of the window is
+ *                        NaN, whatever skipna is (window > ntime: all NaN)
+ *   +-Inf                as NumPy float64 over the window: mean([1, inf]) = inf,
+ *                        inf + -inf = nan; a window that slid past an Inf is finite
+ * Mean and sum accumulate in float64; min and max are one of the window's values.
+ *   mean, min, max, sum  device [nouter][nout][ninner] of x's dtype (nout = nbin,
+ *                        or ntime for rolling); NULL = not wanted, at least one
+ *                        given                                                       */
+int wb2_time_window_stats(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter,
+                          int64_t ntime, int64_t ninner, int64_t nbin,
+                          const int64_t* bin_start, const int32_t* bin_count,
+                          int32_t window, int skipna, void* mean, void* min, void* max,
+                          void* sum);
+
+/* wb2_time_window_stats on a HOST series (NumPy / memmap): bands of inner cells of
+ * one outer index (or of whole outer indices when they fit), each band in one
+ * strided 2-D copy, double buffered so that the copy of band b+1 overlaps the
+ * kernel of band b; every output band is copied back.  `budget` bounds the device
+ * bytes of the two staging buffers (at least one cell per band).  mean / min /
+ * max / sum are host arrays of the same layout.                                    */
+int wb2_time_window_stats_host(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter,
+                               int64_t ntime, int64_t ninner, int64_t nbin,
+                               const int64_t* bin_start, const int32_t* bin_count,
+                               int32_t window, int skipna, size_t budget, void* mean,
+                               void* min, void* max, void* sum);
+
 /* ---- K10: rank histogram ---------------------------------------------------------
  * Replaces RankHistogram.compute_chunk (metrics.py:1894-2042) and the time mean
  * of EnsembleMetric.compute: rank of the truth among the members (NaN last),

@@ -184,6 +184,12 @@ PROTOTYPES = {
         C.c_int32, C.c_int32, C.c_int32, _I64P, _I64P, _I32P, _I32P, C.c_int32,
         C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_int32, C.c_double,
         C.c_size_t, _P, _P]),
+    'wb2_time_window_stats': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I64P,
+        _I32P, C.c_int32, C.c_int, _P, _P, _P, _P]),
+    'wb2_time_window_stats_host': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I64P,
+        _I32P, C.c_int32, C.c_int, C.c_size_t, _P, _P, _P, _P]),
 }
 # wb2_climatology_quantile: quantiles per call, nitem * window_size per window
 CLIM_MAX_QUANTILES = 16
@@ -672,6 +678,42 @@ class Context:
         self.handle, _P(x), dtype, int(ntime), int(ncell),
         *self._climatology_args(plan)[:-1], *args, int(budget), _P(out),
         _P(dry_fraction) if dry_fraction else None))
+    del keep
+
+  # -- time resampling / rolling windows ---------------------------------------
+  @staticmethod
+  def _time_window_args(bin_start, bin_count):
+    s = None if bin_start is None else np.ascontiguousarray(bin_start,
+                                                            dtype=np.int64)
+    c = None if bin_count is None else np.ascontiguousarray(bin_count,
+                                                            dtype=np.int32)
+    nbin = s.size if s is not None else (c.size if c is not None else 0)
+    return (int(nbin), _as_ptr(s, C.c_int64), _as_ptr(c, C.c_int32)), (s, c)
+
+  def time_window_stats(self, x: int, dtype: int, nouter: int, ntime: int,
+                        ninner: int, bin_start, bin_count, window: int,
+                        skipna: bool, mean: Optional[int], min: Optional[int],  # pylint: disable=redefined-builtin
+                        max: Optional[int], sum: Optional[int]):  # pylint: disable=redefined-builtin
+    """x and the outputs are DEVICE addresses (wb2_time_window_stats);
+    bin_start / bin_count host arrays (resample) or None (rolling window)."""
+    args, keep = self._time_window_args(bin_start, bin_count)
+    check(self.lib.wb2_time_window_stats(
+        self.handle, _P(x), dtype, int(nouter), int(ntime), int(ninner), *args,
+        int(window), int(bool(skipna)), *(_P(p) if p else None
+                                          for p in (mean, min, max, sum))))
+    del keep
+
+  def time_window_stats_host(self, x: int, dtype: int, nouter: int,
+                             ntime: int, ninner: int, bin_start, bin_count,
+                             window: int, skipna: bool, budget: int,
+                             mean: Optional[int], min: Optional[int],  # pylint: disable=redefined-builtin
+                             max: Optional[int], sum: Optional[int]):  # pylint: disable=redefined-builtin
+    """x and the outputs are HOST addresses (wb2_time_window_stats_host)."""
+    args, keep = self._time_window_args(bin_start, bin_count)
+    check(self.lib.wb2_time_window_stats_host(
+        self.handle, _P(x), dtype, int(nouter), int(ntime), int(ninner), *args,
+        int(window), int(bool(skipna)), int(budget),
+        *(_P(p) if p else None for p in (mean, min, max, sum))))
     del keep
 
   # -- K10 --------------------------------------------------------------------
