@@ -278,35 +278,27 @@ int clim_validate(int64_t ntime, int64_t nres, const int64_t* res_start,
   return WB2_OK;
 }
 
-// One device block (a Packer slot could be recycled by the wb2_ens_mean calls
-// of the resample).
 int clim_upload(wb2_ctx* ctx, const ClimPlan& p, const int64_t* items, const int64_t* fill,
-                ClimDeviceTables* t) {
-  const size_t n_items = size_t(p.nhour) * p.nday * p.nitem;
+                DeviceBlock* blk, ClimArgs* a) {
   const size_t n_fill = p.fill ? size_t(p.nhour) * p.nitem : 0;
-  const size_t o_fill = n_items * 8;
-  const size_t o_nday = o_fill + n_fill * 8;
-  const size_t o_row = o_nday + (size_t(p.nhour) * 4 + 7) / 8 * 8;
-  const size_t bytes = o_row + size_t(p.nhour) * p.nday * 4;
-  std::vector<char> h(bytes);
-  memcpy(h.data(), items, n_items * 8);
-  if (n_fill) memcpy(h.data() + o_fill, fill, n_fill * 8);
-  memcpy(h.data() + o_nday, p.hour_nday, size_t(p.nhour) * 4);
-  memcpy(h.data() + o_row, p.out_row, size_t(p.nhour) * p.nday * 4);
-  WB2_CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&t->base), bytes, ctx->stream));
-  WB2_CUDA_TRY(cudaMemcpyAsync(t->base, h.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
-  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // `h` is pageable and goes away
-  ClimArgs& a = t->args;
-  a.items = reinterpret_cast<const int64_t*>(t->base);
-  a.fill = n_fill ? reinterpret_cast<const int64_t*>(t->base + o_fill) : nullptr;
-  a.hour_nday = reinterpret_cast<const int32_t*>(t->base + o_nday);
-  a.out_row = reinterpret_cast<const int32_t*>(t->base + o_row);
-  a.nhour = p.nhour;
-  a.nday = p.nday;
-  a.nitem = p.nitem;
-  a.nday_out = p.nday_out;
-  a.half = p.half;
-  a.fast = p.fast;
+  size_t o[4];
+  WB2_TRY(upload_parts(ctx,
+                       {{items, size_t(p.nhour) * p.nday * p.nitem * 8},
+                        {fill, n_fill * 8},
+                        {p.hour_nday, size_t(p.nhour) * 4},
+                        {p.out_row, size_t(p.nhour) * p.nday * 4}},
+                       blk, o));
+  *a = ClimArgs{};
+  a->items = blk->at<const int64_t>(o[0]);
+  a->fill = n_fill ? blk->at<const int64_t>(o[1]) : nullptr;
+  a->hour_nday = blk->at<const int32_t>(o[2]);
+  a->out_row = blk->at<const int32_t>(o[3]);
+  a->nhour = p.nhour;
+  a->nday = p.nday;
+  a->nitem = p.nitem;
+  a->nday_out = p.nday_out;
+  a->half = p.half;
+  a->fast = p.fast;
   return WB2_OK;
 }
 
@@ -415,65 +407,44 @@ int clim_stream_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime, int6
   size_t stage_bytes = b_in + b_day;
   for (int s = 0; s < nout; ++s) stage_bytes += b_out[size_t(s)] = al(out_rows[s] * nb * 4);
 
-  ClimDeviceTables t;
-  char* stage[2] = {nullptr, nullptr};
-  const int rc = [&]() -> int {
-    WB2_TRY(clim_upload(ctx, p, it_r.data(), n_fill ? fill_r.data() : nullptr, &t));
-    for (int i = 0; i < 2; ++i)
-      WB2_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&stage[i]), stage_bytes));
-    const char* xh = static_cast<const char*>(x);
-    bool used[2] = {false, false};
-    int buf = 0;
-    std::vector<float*> out(static_cast<size_t>(nout));
-    for (int64_t c0 = 0; c0 < ncell; c0 += nb) {
-      const int64_t n = std::min(nb, ncell - c0);
-      char* in = stage[buf];
-      float* daily = reinterpret_cast<float*>(in + b_in);
-      char* o = in + b_in + b_day;
-      for (int s = 0; s < nout; ++s) {
-        out[size_t(s)] = reinterpret_cast<float*>(o);
-        o += b_out[size_t(s)];
-      }
-      if (used[buf])
-        WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
-      if (rows > 0) {  // the band's whole selected series: one strided 2-D copy
-        WB2_CUDA_TRY(cudaMemcpy2DAsync(in, size_t(n) * esize,
-                                       xh + (size_t(t_lo) * ncell + c0) * esize,
-                                       size_t(ncell) * esize, size_t(n) * esize, size_t(rows),
-                                       cudaMemcpyHostToDevice, ctx->copy_stream));
-        ctx->stat_h2d_bytes += rows * n * int64_t(esize);
-      }
-      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
-      WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
-      const void* src = in;
-      if (nres > 0) {
-        WB2_TRY(clim_resample(ctx, reinterpret_cast<const float*>(in), n, n, p, start_r.data(),
-                              daily));
-        src = daily;
-      }
-      if (p.need_nan_fill)
-        WB2_CUDA_TRY(cudaMemsetAsync(out[0], 0xFF, size_t(o - reinterpret_cast<char*>(out[0])),
-                                     ctx->stream));
-      WB2_TRY(band(src, n, t.args, out.data()));
-      for (int s = 0; s < nout; ++s) {
-        WB2_CUDA_TRY(cudaMemcpy2DAsync(out_host[s] + c0, size_t(ncell) * 4, out[size_t(s)],
-                                       size_t(n) * 4, size_t(n) * 4, out_rows[s],
-                                       cudaMemcpyDeviceToHost, ctx->stream));
-        ctx->stat_d2h_bytes += int64_t(out_rows[s]) * n * 4;
-      }
-      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
-      used[buf] = true;
-      buf ^= 1;
+  DeviceBlock tables;
+  ClimArgs args;
+  WB2_TRY(clim_upload(ctx, p, it_r.data(), n_fill ? fill_r.data() : nullptr, &tables, &args));
+  StagePair stage;
+  WB2_TRY(stage.alloc(stage_bytes));
+  StagePipe pipe(ctx, stage.buf[0], stage.buf[1]);
+  const char* xh = static_cast<const char*>(x);
+  std::vector<float*> out(static_cast<size_t>(nout));
+  for (int64_t c0 = 0; c0 < ncell; c0 += nb) {
+    const int64_t n = std::min(nb, ncell - c0);
+    char* in;
+    WB2_TRY(pipe.next(&in));
+    float* daily = reinterpret_cast<float*>(in + b_in);
+    char* o = in + b_in + b_day;
+    for (int s = 0; s < nout; ++s) {
+      out[size_t(s)] = reinterpret_cast<float*>(o);
+      o += b_out[size_t(s)];
     }
-    WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return WB2_OK;
-  }();
-  cudaStreamSynchronize(ctx->stream);
-  cudaStreamSynchronize(ctx->copy_stream);
-  for (int i = 0; i < 2; ++i)
-    if (stage[i]) cudaFree(stage[i]);
-  if (t.base) cudaFree(t.base);
-  return rc;
+    if (rows > 0)  // the band's whole selected series: one strided 2-D copy
+      WB2_TRY(pipe.h2d_2d(in, size_t(n) * esize, xh + (size_t(t_lo) * ncell + c0) * esize,
+                          size_t(ncell) * esize, size_t(n) * esize, size_t(rows)));
+    WB2_TRY(pipe.ready());
+    const void* src = in;
+    if (nres > 0) {
+      WB2_TRY(clim_resample(ctx, reinterpret_cast<const float*>(in), n, n, p, start_r.data(),
+                            daily));
+      src = daily;
+    }
+    if (p.need_nan_fill)
+      WB2_CUDA_TRY(cudaMemsetAsync(out[0], 0xFF, size_t(o - reinterpret_cast<char*>(out[0])),
+                                   ctx->stream));
+    WB2_TRY(band(src, n, args, out.data()));
+    for (int s = 0; s < nout; ++s)
+      WB2_TRY(pipe.d2h_2d(out_host[s] + c0, size_t(ncell) * 4, out[size_t(s)], size_t(n) * 4,
+                          size_t(n) * 4, out_rows[s]));
+    WB2_TRY(pipe.done());
+  }
+  return pipe.finish();
 }
 
 }  // namespace wb2
@@ -500,28 +471,22 @@ int wb2_climatology(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime, int64
   if (ncell == 0) return WB2_OK;
   WB2_REQUIRE(x != nullptr, "x is NULL");
   DeviceGuard guard(ctx->device);
-  ClimDeviceTables t;
-  float* daily = nullptr;
-  const int rc = [&]() -> int {
-    WB2_TRY(clim_upload(ctx, p, items, p.fill, &t));
-    const void* src = x;
-    if (nres > 0) {
-      WB2_CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&daily),
-                                   size_t(nres) * ncell * 4, ctx->stream));
-      WB2_TRY(clim_resample(ctx, static_cast<const float*>(x), ncell, ncell, p, res_start,
-                            daily));
-      src = daily;
-    }
-    const size_t out_bytes = size_t(nhour) * nday_out * ncell * 4;
-    if (p.need_nan_fill) {  // day labels some hour does not have
-      if (mean) WB2_CUDA_TRY(cudaMemsetAsync(mean, 0xFF, out_bytes, ctx->stream));
-      if (std) WB2_CUDA_TRY(cudaMemsetAsync(std, 0xFF, out_bytes, ctx->stream));
-    }
-    return clim_launch(ctx, src, dtype, ncell, ncell, t.args, mean, std);
-  }();
-  if (daily) cudaFreeAsync(daily, ctx->stream);
-  if (t.base) cudaFreeAsync(t.base, ctx->stream);
-  return rc;
+  DeviceBlock tables, daily;
+  ClimArgs args;
+  WB2_TRY(clim_upload(ctx, p, items, p.fill, &tables, &args));
+  const void* src = x;
+  if (nres > 0) {
+    WB2_TRY(daily.alloc(ctx, size_t(nres) * ncell * 4));
+    WB2_TRY(clim_resample(ctx, static_cast<const float*>(x), ncell, ncell, p, res_start,
+                          daily.at<float>(0)));
+    src = daily.at<float>(0);
+  }
+  const size_t out_bytes = size_t(nhour) * nday_out * ncell * 4;
+  if (p.need_nan_fill) {  // day labels some hour does not have
+    if (mean) WB2_CUDA_TRY(cudaMemsetAsync(mean, 0xFF, out_bytes, ctx->stream));
+    if (std) WB2_CUDA_TRY(cudaMemsetAsync(std, 0xFF, out_bytes, ctx->stream));
+  }
+  return clim_launch(ctx, src, dtype, ncell, ncell, args, mean, std);
 }
 
 int wb2_climatology_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime, int64_t ncell,

@@ -1,12 +1,12 @@
 // Shared host side of the day-of-year climatology entries (climatology.cu and
 // climatology_quantile.cu): the validated index tables, their device copy, the
-// daily resample and the band loop that streams a host series through the
-// double-buffered staging of the context.
+// daily resample and the band loop that streams a host series through a
+// StagePipe (stage.cuh).
 #pragma once
 
 #include <functional>
 
-#include "common.cuh"
+#include "stage.cuh"
 
 namespace wb2 {
 
@@ -43,14 +43,10 @@ int clim_validate(int64_t ntime, int64_t nres, const int64_t* res_start,
                   const int32_t* out_row, int32_t nday_out, int32_t window_size,
                   int32_t method, ClimPlan* p);
 
-// Device copy of the tables: [items][fill][hour_nday][out_row] in one block.
-struct ClimDeviceTables {
-  char* base = nullptr;
-  ClimArgs args{};
-};
-
+// Device copy of the tables, [items][fill][hour_nday][out_row] in `blk`; `a`
+// gets their device pointers and the plan's sizes.
 int clim_upload(wb2_ctx* ctx, const ClimPlan& p, const int64_t* items, const int64_t* fill,
-                ClimDeviceTables* t);
+                DeviceBlock* blk, ClimArgs* a);
 
 // resample(time='D').mean() of a device series into `daily` [nres][ncell].
 int clim_resample(wb2_ctx* ctx, const float* x, int64_t tstride, int64_t ncell,
@@ -63,10 +59,10 @@ int clim_resample(wb2_ctx* ctx, const float* x, int64_t tstride, int64_t ncell,
 using ClimBandFn =
     std::function<int(const void* src, int64_t n, const ClimArgs& tables, float* const* out)>;
 
-// The band loop of the *_host entries: bands of cells sized so that the two
-// staging buffers (selected input rows, resampled days and `nout` outputs of
-// out_rows[s] rows each) fit `budget`; one strided 2-D copy per band on the
-// copy stream overlaps the previous band's kernels; every output band is
+// The band loop of the *_host entries: bands of cells sized so that a private
+// StagePair (selected input rows, resampled days and `nout` outputs of
+// out_rows[s] rows each) fits `budget`; through a StagePipe, one strided 2-D
+// copy per band overlaps the previous band's kernels; every output band is
 // copied back into out_host[s] ([out_rows[s]][ncell]).
 int clim_stream_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime, int64_t ncell,
                      const ClimPlan& p, size_t budget, int nout, float* const* out_host,

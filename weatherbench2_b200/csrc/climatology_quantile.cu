@@ -340,7 +340,7 @@ static int quant_prepare(wb2_ctx* ctx, int dtype, int64_t ncell, int64_t nres, i
                          int32_t nday, int32_t nitem, const int64_t* items,
                          const int32_t* hour_nday, int32_t window_size, int32_t nq,
                          const double* quantiles, int32_t seeps, double dry_threshold,
-                         const float* dry_fraction, QuantArgs* q, double** block_dev) {
+                         const float* dry_fraction, QuantArgs* q, DeviceBlock* blk) {
   WB2_REQUIRE(dtype == WB2_F32 || dtype == WB2_F64, "dtype must be WB2_F32 or WB2_F64");
   WB2_REQUIRE(nres == 0 || dtype == WB2_F32, "nres > 0 (the daily resample) takes float32 input");
   WB2_REQUIRE(ncell >= 0, "ncell < 0");
@@ -360,25 +360,20 @@ static int quant_prepare(wb2_ctx* ctx, int dtype, int64_t ncell, int64_t nres, i
   q->nq = nq;
   q->seeps = seeps;
   q->dry = dry_threshold;
-  // [quantiles][stacked years of each hour: the item columns that hold any step]
-  std::vector<double> blk(size_t(nq) + (size_t(nhour) + 1) / 2, 0.0);
-  std::copy(quantiles, quantiles + nq, blk.begin());
-  int32_t* ny = reinterpret_cast<int32_t*>(blk.data() + nq);
+  // stacked years of each hour: the item columns that hold any step
+  std::vector<int32_t> ny(size_t(nhour), 0);
   for (int32_t h = 0; h < nhour; ++h)
     for (int32_t j = 0; j < nitem; ++j)
       for (int32_t d = 0; d < hour_nday[h]; ++d)
         if (items[(int64_t(h) * nday + d) * nitem + j] >= 0) {
-          ny[h] += 1;
+          ny[size_t(h)] += 1;
           break;
         }
   if (ncell == 0) return WB2_OK;
-  const size_t bytes = blk.size() * 8;
-  WB2_CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(block_dev), bytes, ctx->stream));
-  WB2_CUDA_TRY(
-      cudaMemcpyAsync(*block_dev, blk.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
-  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // `blk` is pageable and goes away
-  q->q = *block_dev;
-  q->hour_nyear = reinterpret_cast<const int32_t*>(*block_dev + nq);
+  size_t o[2];
+  WB2_TRY(upload_parts(ctx, {{quantiles, size_t(nq) * 8}, {ny.data(), ny.size() * 4}}, blk, o));
+  q->q = blk->at<const double>(o[0]);
+  q->hour_nyear = blk->at<const int32_t>(o[1]);
   return WB2_OK;
 }
 
@@ -404,35 +399,27 @@ int wb2_climatology_quantile(wb2_ctx* ctx, const void* x, int dtype, int64_t nti
   WB2_REQUIRE(out != nullptr || ncell == 0, "out is NULL");
   DeviceGuard guard(ctx->device);
   QuantArgs q;
-  double* nyear = nullptr;
-  ClimDeviceTables t;
-  float* daily = nullptr;
-  const int rc = [&]() -> int {
-    WB2_TRY(quant_prepare(ctx, dtype, ncell, nres, nhour, nday, nitem, items, hour_nday,
-                          window_size, nquantile, quantiles, seeps, dry_threshold, dry_fraction,
-                          &q, &nyear));
-    if (ncell == 0) return WB2_OK;
-    WB2_REQUIRE(x != nullptr, "x is NULL");
-    WB2_TRY(clim_upload(ctx, p, items, p.fill, &t));
-    const void* src = x;
-    if (nres > 0) {
-      WB2_CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&daily),
-                                   size_t(nres) * ncell * 4, ctx->stream));
-      WB2_TRY(clim_resample(ctx, static_cast<const float*>(x), ncell, ncell, p, res_start,
-                            daily));
-      src = daily;
-    }
-    if (p.need_nan_fill) {  // day labels some hour does not have
-      const size_t rows = size_t(nhour) * nday_out * ncell * 4;
-      WB2_CUDA_TRY(cudaMemsetAsync(out, 0xFF, rows * nquantile, ctx->stream));
-      if (dry_fraction) WB2_CUDA_TRY(cudaMemsetAsync(dry_fraction, 0xFF, rows, ctx->stream));
-    }
-    return quant_launch(ctx, src, dtype, ncell, t.args, q, out, dry_fraction);
-  }();
-  if (daily) cudaFreeAsync(daily, ctx->stream);
-  if (t.base) cudaFreeAsync(t.base, ctx->stream);
-  if (nyear) cudaFreeAsync(nyear, ctx->stream);
-  return rc;
+  DeviceBlock nyear, tables, daily;
+  WB2_TRY(quant_prepare(ctx, dtype, ncell, nres, nhour, nday, nitem, items, hour_nday,
+                        window_size, nquantile, quantiles, seeps, dry_threshold, dry_fraction, &q,
+                        &nyear));
+  if (ncell == 0) return WB2_OK;
+  WB2_REQUIRE(x != nullptr, "x is NULL");
+  ClimArgs args;
+  WB2_TRY(clim_upload(ctx, p, items, p.fill, &tables, &args));
+  const void* src = x;
+  if (nres > 0) {
+    WB2_TRY(daily.alloc(ctx, size_t(nres) * ncell * 4));
+    WB2_TRY(clim_resample(ctx, static_cast<const float*>(x), ncell, ncell, p, res_start,
+                          daily.at<float>(0)));
+    src = daily.at<float>(0);
+  }
+  if (p.need_nan_fill) {  // day labels some hour does not have
+    const size_t rows = size_t(nhour) * nday_out * ncell * 4;
+    WB2_CUDA_TRY(cudaMemsetAsync(out, 0xFF, rows * nquantile, ctx->stream));
+    if (dry_fraction) WB2_CUDA_TRY(cudaMemsetAsync(dry_fraction, 0xFF, rows, ctx->stream));
+  }
+  return quant_launch(ctx, src, dtype, ncell, args, q, out, dry_fraction);
 }
 
 int wb2_climatology_quantile_host(wb2_ctx* ctx, const void* x, int dtype, int64_t ntime,
@@ -452,27 +439,20 @@ int wb2_climatology_quantile_host(wb2_ctx* ctx, const void* x, int dtype, int64_
   WB2_REQUIRE(out_host != nullptr || ncell == 0, "out is NULL");
   DeviceGuard guard(ctx->device);
   QuantArgs q;
-  double* nyear = nullptr;
-  const int rc = [&]() -> int {
-    WB2_TRY(quant_prepare(ctx, dtype, ncell, nres, nhour, nday, nitem, items, hour_nday,
-                          window_size, nquantile, quantiles, seeps, dry_threshold,
-                          dry_fraction_host, &q, &nyear));
-    if (ncell == 0) return WB2_OK;
-    WB2_REQUIRE(x != nullptr, "x is NULL");
-    float* const out[2] = {out_host, dry_fraction_host};
-    const size_t rows = size_t(nhour) * nday_out;
-    const size_t out_rows[2] = {rows * nquantile, rows};
-    return clim_stream_host(
-        ctx, x, dtype, ntime, ncell, p, budget, seeps ? 2 : 1, out, out_rows,
-        [&](const void* src, int64_t n, const ClimArgs& tables, float* const* o) {
-          return quant_launch(ctx, src, dtype, n, tables, q, o[0], seeps ? o[1] : nullptr);
-        });
-  }();
-  if (nyear) {
-    cudaFreeAsync(nyear, ctx->stream);
-    cudaStreamSynchronize(ctx->stream);
-  }
-  return rc;
+  DeviceBlock nyear;
+  WB2_TRY(quant_prepare(ctx, dtype, ncell, nres, nhour, nday, nitem, items, hour_nday,
+                        window_size, nquantile, quantiles, seeps, dry_threshold,
+                        dry_fraction_host, &q, &nyear));
+  if (ncell == 0) return WB2_OK;
+  WB2_REQUIRE(x != nullptr, "x is NULL");
+  float* const out[2] = {out_host, dry_fraction_host};
+  const size_t rows = size_t(nhour) * nday_out;
+  const size_t out_rows[2] = {rows * nquantile, rows};
+  return clim_stream_host(
+      ctx, x, dtype, ntime, ncell, p, budget, seeps ? 2 : 1, out, out_rows,
+      [&](const void* src, int64_t n, const ClimArgs& tables, float* const* o) {
+        return quant_launch(ctx, src, dtype, n, tables, q, o[0], seeps ? o[1] : nullptr);
+      });
 }
 
 }  // extern "C"

@@ -18,7 +18,7 @@
 #include <algorithm>
 #include <unordered_map>
 
-#include "common.cuh"
+#include "stage.cuh"
 
 namespace wb2 {
 
@@ -231,11 +231,11 @@ int wb2_det_metrics_host(wb2_ctx* ctx, const void* f, const void* t, const void*
   struct Copy { const char* src; char* dst; };
   std::vector<int64_t> loc[3];
   std::vector<Copy> copies;
-  int buf = 0;
+  StagePipe pipe(ctx, ctx->stage[0], ctx->stage[1]);
   int64_t g0 = 0;
-  bool used[2] = {false, false};
   while (g0 < nfield) {
-    char* stage = static_cast<char*>(ctx->stage[buf]);
+    char* stage;
+    WB2_TRY(pipe.next(&stage));
     const uint64_t tick = cache ? cache->tick++ : 0;
     bool wait_prev_group = false;
     std::unordered_map<const char*, int64_t> slot_of;  // staged host address -> staging slot
@@ -284,31 +284,18 @@ int wb2_det_metrics_host(wb2_ctx* ctx, const void* f, const void* t, const void*
       ++g1;
     }
     WB2_REQUIRE(g1 > g0, "staging buffer too small for one field");
-    if (used[buf]) WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
-    if (wait_prev_group && used[buf ^ 1])  // an evicted slot was read by the previous group
-      WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf ^ 1], 0));
-    for (const Copy& cp : copies)
-      WB2_CUDA_TRY(cudaMemcpyAsync(cp.dst, cp.src, copy_bytes, cudaMemcpyHostToDevice,
-                                   ctx->copy_stream));
-    ctx->stat_h2d_bytes += int64_t(copies.size()) * int64_t(copy_bytes);
-    WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
-    WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
-    int rc = det_metrics_impl(ctx, c ? 1 : 0, stage, stage, c ? stage : nullptr, nullptr, dtype,
-                              g1 - g0, loc[0].data(), loc[1].data(),
-                              c ? loc[2].data() : nullptr, nullptr, w, skipna,
-                              ctx->d_out_tmp + size_t(g0) * per_field);
-    if (rc != WB2_OK) return rc;
-    WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
-    used[buf] = true;
-    buf ^= 1;
+    if (wait_prev_group) WB2_TRY(pipe.wait_other());  // an evicted slot was read by it
+    for (const Copy& cp : copies) WB2_TRY(pipe.h2d(cp.dst, cp.src, copy_bytes));
+    WB2_TRY(pipe.ready());
+    WB2_TRY(det_metrics_impl(ctx, c ? 1 : 0, stage, stage, c ? stage : nullptr, nullptr, dtype,
+                             g1 - g0, loc[0].data(), loc[1].data(),
+                             c ? loc[2].data() : nullptr, nullptr, w, skipna,
+                             ctx->d_out_tmp + size_t(g0) * per_field));
+    WB2_TRY(pipe.done());
     g0 = g1;
   }
-  const size_t out_bytes = size_t(nfield) * per_field * sizeof(double);
-  WB2_CUDA_TRY(cudaMemcpyAsync(out_host, ctx->d_out_tmp, out_bytes, cudaMemcpyDeviceToHost,
-                               ctx->stream));
-  ctx->stat_d2h_bytes += int64_t(out_bytes);
-  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  return WB2_OK;
+  WB2_TRY(pipe.d2h(out_host, ctx->d_out_tmp, size_t(nfield) * per_field * sizeof(double)));
+  return pipe.finish();
 }
 
 // ---- K2 -----------------------------------------------------------------------
@@ -345,14 +332,13 @@ int wb2_ens_metrics_host(wb2_ctx* ctx, const void* x, const void* t, int dtype,
   const char* xh = static_cast<const char*>(x);
   const char* th = static_cast<const char*>(t);
   std::vector<int64_t> lx, lt;
-  int buf = 0;
-  bool used[2] = {false, false};
+  StagePipe pipe(ctx, ctx->stage[0], ctx->stage[1]);
   for (int64_t g0 = 0; g0 < nfield; g0 += fields_per_group) {
     const int64_t g1 = std::min(nfield, g0 + fields_per_group);
-    char* stage = static_cast<char*>(ctx->stage[buf]);
+    char* stage;
+    WB2_TRY(pipe.next(&stage));
     const uint64_t tick = cache ? cache->tick++ : 0;
     bool wait_prev_group = false;
-    if (used[buf]) WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
     lx.clear();
     lt.clear();
     struct Copy { const char* src; char* dst; };
@@ -360,10 +346,9 @@ int wb2_ens_metrics_host(wb2_ctx* ctx, const void* x, const void* t, int dtype,
     for (int64_t i = g0; i < g1; ++i) {
       char* fbase = stage + size_t(i - g0) * size_t(per) * slab_bytes;
       for (int m = 0; m < nmember; ++m)
-        WB2_CUDA_TRY(cudaMemcpyAsync(fbase + size_t(m) * slab_bytes,
-                                     xh + (off_x[i] + int64_t(m) * member_stride) * int64_t(esize),
-                                     copy_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
-      ctx->stat_h2d_bytes += int64_t(nmember) * int64_t(copy_bytes);
+        WB2_TRY(pipe.h2d(fbase + size_t(m) * slab_bytes,
+                         xh + (off_x[i] + int64_t(m) * member_stride) * int64_t(esize),
+                         copy_bytes));
       lx.push_back((fbase - stage) / int64_t(esize));
       const char* tsrc = th + off_t[i] * int64_t(esize);
       char* tdev = nullptr;
@@ -388,27 +373,15 @@ int wb2_ens_metrics_host(wb2_ctx* ctx, const void* x, const void* t, int dtype,
       }
       lt.push_back((tdev - stage) / int64_t(esize));
     }
-    if (wait_prev_group && used[buf ^ 1])
-      WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf ^ 1], 0));
-    for (const Copy& cp : late)
-      WB2_CUDA_TRY(cudaMemcpyAsync(cp.dst, cp.src, copy_bytes, cudaMemcpyHostToDevice,
-                                   ctx->copy_stream));
-    ctx->stat_h2d_bytes += int64_t(late.size()) * int64_t(copy_bytes);
-    WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
-    WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
-    int rc = wb2_ens_metrics(ctx, stage, stage, WB2_F32, nmember, slab_pad, g1 - g0, lx.data(),
-                             lt.data(), w, skipna, ctx->d_out_tmp + size_t(g0) * per_field);
-    if (rc != WB2_OK) return rc;
-    WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
-    used[buf] = true;
-    buf ^= 1;
+    if (wait_prev_group) WB2_TRY(pipe.wait_other());
+    for (const Copy& cp : late) WB2_TRY(pipe.h2d(cp.dst, cp.src, copy_bytes));
+    WB2_TRY(pipe.ready());
+    WB2_TRY(wb2_ens_metrics(ctx, stage, stage, WB2_F32, nmember, slab_pad, g1 - g0, lx.data(),
+                            lt.data(), w, skipna, ctx->d_out_tmp + size_t(g0) * per_field));
+    WB2_TRY(pipe.done());
   }
-  const size_t out_bytes = size_t(nfield) * per_field * sizeof(double);
-  WB2_CUDA_TRY(cudaMemcpyAsync(out_host, ctx->d_out_tmp, out_bytes, cudaMemcpyDeviceToHost,
-                               ctx->stream));
-  ctx->stat_d2h_bytes += int64_t(out_bytes);
-  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  return WB2_OK;
+  WB2_TRY(pipe.d2h(out_host, ctx->d_out_tmp, size_t(nfield) * per_field * sizeof(double)));
+  return pipe.finish();
 }
 
 // ---- K5 -----------------------------------------------------------------------
@@ -432,31 +405,22 @@ int wb2_regrid_conservative_host(wb2_ctx* ctx, const float* src, float* dst, int
   if (cap < per) cap = per;
   WB2_TRY(ensure_stage(ctx, cap));
   const int64_t fpg = std::max<int64_t>(1, int64_t(ctx->stage_cap / per));
-  int buf = 0;
-  bool used[2] = {false, false};
+  StagePipe pipe(ctx, ctx->stage[0], ctx->stage[1]);
   for (int64_t g0 = 0; g0 < nfield; g0 += fpg) {
     const int64_t n = std::min(fpg, nfield - g0);
-    float* sin = static_cast<float*>(ctx->stage[buf]);
+    float* sin;
+    WB2_TRY(pipe.next(&sin));
     float* sout = sin + size_t(n) * in_pad;
-    if (used[buf]) WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
     // one 2-D copy for the whole group (pitch = the caller's field stride)
-    WB2_CUDA_TRY(cudaMemcpy2DAsync(sin, size_t(in_pad) * 4, src + g0 * src_field_stride,
-                                   size_t(src_field_stride) * 4, size_t(in_elems) * 4, size_t(n),
-                                   cudaMemcpyHostToDevice, ctx->copy_stream));
-    ctx->stat_h2d_bytes += n * in_elems * 4;
-    WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
-    WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
+    WB2_TRY(pipe.h2d_2d(sin, size_t(in_pad) * 4, src + g0 * src_field_stride,
+                        size_t(src_field_stride) * 4, size_t(in_elems) * 4, size_t(n)));
+    WB2_TRY(pipe.ready());
     WB2_TRY(wb2_regrid_conservative(ctx, sin, sout, n, in_pad, out_pad, lon_w, lat_w));
-    WB2_CUDA_TRY(cudaMemcpy2DAsync(dst + g0 * dst_field_stride, size_t(dst_field_stride) * 4,
-                                   sout, size_t(out_pad) * 4, size_t(out_elems) * 4, size_t(n),
-                                   cudaMemcpyDeviceToHost, ctx->stream));
-    ctx->stat_d2h_bytes += n * out_elems * 4;
-    WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
-    used[buf] = true;
-    buf ^= 1;
+    WB2_TRY(pipe.d2h_2d(dst + g0 * dst_field_stride, size_t(dst_field_stride) * 4, sout,
+                        size_t(out_pad) * 4, size_t(out_elems) * 4, size_t(n)));
+    WB2_TRY(pipe.done());
   }
-  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  return WB2_OK;
+  return pipe.finish();
 }
 
 // ---- K4 -----------------------------------------------------------------------
@@ -490,29 +454,20 @@ static int spectrum_host(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t n
     if (cap < per) cap = per;
     WB2_TRY(ensure_stage(ctx, cap));
     const int64_t fpg = std::max<int64_t>(1, int64_t(ctx->stage_cap / per));
-    int buf = 0;
-    bool used[2] = {false, false};
+    StagePipe pipe(ctx, ctx->stage[0], ctx->stage[1]);
     for (int64_t g0 = 0; g0 < nfield; g0 += fpg) {
       const int64_t n = std::min(fpg, nfield - g0);
-      float* sin = static_cast<float*>(ctx->stage[buf]);
-      if (used[buf]) WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
+      float* sin;
+      WB2_TRY(pipe.next(&sin));
       // rows stay contiguous: in_elems per field, no padding between fields
-      WB2_CUDA_TRY(cudaMemcpyAsync(sin, x + g0 * in_elems, size_t(n) * in_elems * 4,
-                                   cudaMemcpyHostToDevice, ctx->copy_stream));
-      ctx->stat_h2d_bytes += n * in_elems * 4;
-      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
-      WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
+      WB2_TRY(pipe.h2d(sin, x + g0 * in_elems, size_t(n) * in_elems * 4));
+      WB2_TRY(pipe.ready());
       float* sout = sin + (size_t(n) * in_elems + 63) / 64 * 64;
       WB2_TRY(wb2_zonal_spectrum(ctx, sin, n, nrow, ncol, scale, sout, 0, n));
-      WB2_CUDA_TRY(cudaMemcpyAsync(out_host + g0 * out_elems, sout, size_t(n) * out_elems * 4,
-                                   cudaMemcpyDeviceToHost, ctx->stream));
-      ctx->stat_d2h_bytes += n * out_elems * 4;
-      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
-      used[buf] = true;
-      buf ^= 1;
+      WB2_TRY(pipe.d2h(out_host + g0 * out_elems, sout, size_t(n) * out_elems * 4));
+      WB2_TRY(pipe.done());
     }
-    WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return WB2_OK;
+    return pipe.finish();
   }
 
   // time-summed / latitude-reduced: the accumulator stays on the device.  A
@@ -529,38 +484,29 @@ static int spectrum_host(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t n
   WB2_TRY(ensure_out_tmp(ctx, acc_bytes));
   float* acc = reinterpret_cast<float*>(ctx->d_out_tmp);
   WB2_CUDA_TRY(cudaMemsetAsync(acc, 0, acc_bytes, ctx->stream));
-  int buf = 0;
-  bool used[2] = {false, false};
+  StagePipe pipe(ctx, ctx->stage[0], ctx->stage[1]);
   for (int64_t s0 = 0; s0 < nfield_out; s0 += S) {
     const int64_t ns = std::min(S, nfield_out - s0);
     for (int64_t t0 = 0; t0 < ntimes; t0 += k) {
       const int64_t nt = std::min(k, ntimes - t0);
-      float* sin = static_cast<float*>(ctx->stage[buf]);
-      if (used[buf]) WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
+      float* sin;
+      WB2_TRY(pipe.next(&sin));
       // per time step a contiguous run of ns fields
       for (int64_t ti = 0; ti < nt; ++ti)
-        WB2_CUDA_TRY(cudaMemcpyAsync(sin + ti * ns * in_elems,
-                                     x + ((t0 + ti) * nfield_out + s0) * in_elems,
-                                     size_t(ns) * in_elems * 4, cudaMemcpyHostToDevice,
-                                     ctx->copy_stream));
-      ctx->stat_h2d_bytes += nt * ns * in_elems * 4;
-      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
-      WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
+        WB2_TRY(pipe.h2d(sin + ti * ns * in_elems, x + ((t0 + ti) * nfield_out + s0) * in_elems,
+                         size_t(ns) * in_elems * 4));
+      WB2_TRY(pipe.ready());
       if (reduce)
         WB2_TRY(spectrum_latsum_impl(ctx, sin, nt * ns, nrow, ncol, scale, acc + s0 * out_elems,
                                      ns, 1));
       else
         WB2_TRY(wb2_zonal_spectrum(ctx, sin, nt * ns, nrow, ncol, scale, acc + s0 * out_elems,
                                    1, ns));
-      WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
-      used[buf] = true;
-      buf ^= 1;
+      WB2_TRY(pipe.done());
     }
   }
-  WB2_CUDA_TRY(cudaMemcpyAsync(out_host, acc, acc_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-  ctx->stat_d2h_bytes += int64_t(acc_bytes);
-  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  return WB2_OK;
+  WB2_TRY(pipe.d2h(out_host, acc, acc_bytes));
+  return pipe.finish();
 }
 
 int wb2_zonal_spectrum_host(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t nrow,

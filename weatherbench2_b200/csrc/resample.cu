@@ -38,7 +38,7 @@
 
 #include <algorithm>
 
-#include "common.cuh"
+#include "stage.cuh"
 
 namespace wb2 {
 
@@ -327,17 +327,17 @@ static int tw_launch_any(wb2_ctx* ctx, int dtype, const void* x, int64_t nouter,
                    d_count, window, skipna, o);
 }
 
-// Device copy of the bin tables ([start][count] in one block), or nothing.
+// Device copy of the bin tables ([start][count] in `blk`), or NULL pointers
+// when there are none.
 static int tw_upload(wb2_ctx* ctx, int64_t nbin, const int64_t* start, const int32_t* count,
-                     char** base) {
+                     DeviceBlock* blk, const int64_t** d_start, const int32_t** d_count) {
+  *d_start = nullptr;
+  *d_count = nullptr;
   if (nbin == 0 || start == nullptr) return WB2_OK;
-  const size_t bytes = size_t(nbin) * 12;
-  std::vector<char> h(bytes);
-  memcpy(h.data(), start, size_t(nbin) * 8);
-  memcpy(h.data() + size_t(nbin) * 8, count, size_t(nbin) * 4);
-  WB2_CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(base), bytes, ctx->stream));
-  WB2_CUDA_TRY(cudaMemcpyAsync(*base, h.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
-  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));  // `h` is pageable and goes away
+  size_t o[2];
+  WB2_TRY(upload_parts(ctx, {{start, size_t(nbin) * 8}, {count, size_t(nbin) * 4}}, blk, o));
+  *d_start = blk->at<const int64_t>(o[0]);
+  *d_count = blk->at<const int32_t>(o[1]);
   return WB2_OK;
 }
 
@@ -359,18 +359,13 @@ int wb2_time_window_stats(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter
   if (nouter == 0 || ninner == 0 || nout == 0) return WB2_OK;
   WB2_REQUIRE(x != nullptr, "x is NULL");
   DeviceGuard guard(ctx->device);
-  char* tables = nullptr;
   void* const out[4] = {mean, min, max, sum};
-  const int rc = [&]() -> int {
-    WB2_TRY(tw_upload(ctx, nbin, bin_start, bin_count, &tables));
-    const int64_t* d_start = tables ? reinterpret_cast<const int64_t*>(tables) : nullptr;
-    const int32_t* d_count =
-        tables ? reinterpret_cast<const int32_t*>(tables + size_t(nbin) * 8) : nullptr;
-    return tw_launch_any(ctx, dtype, x, nouter, ntime, ninner, nbin, d_start, d_count, window,
-                         skipna, out);
-  }();
-  if (tables) cudaFreeAsync(tables, ctx->stream);
-  return rc;
+  DeviceBlock tables;
+  const int64_t* d_start;
+  const int32_t* d_count;
+  WB2_TRY(tw_upload(ctx, nbin, bin_start, bin_count, &tables, &d_start, &d_count));
+  return tw_launch_any(ctx, dtype, x, nouter, ntime, ninner, nbin, d_start, d_count, window,
+                       skipna, out);
 }
 
 int wb2_time_window_stats_host(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter,
@@ -401,64 +396,42 @@ int wb2_time_window_stats_host(wb2_ctx* ctx, const void* x, int dtype, int64_t n
   const size_t b_in = al(size_t(ko) * nb * ntime * es), b_out = al(size_t(ko) * nb * nout * es);
   const size_t stage_bytes = b_in + nstat * b_out;
 
-  char* tables = nullptr;
-  char* stage[2] = {nullptr, nullptr};
-  const int rc = [&]() -> int {
-    WB2_TRY(tw_upload(ctx, nbin, bin_start, bin_count, &tables));
-    const int64_t* d_start = tables ? reinterpret_cast<const int64_t*>(tables) : nullptr;
-    const int32_t* d_count =
-        tables ? reinterpret_cast<const int32_t*>(tables + size_t(nbin) * 8) : nullptr;
-    for (int i = 0; i < 2; ++i)
-      WB2_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&stage[i]), stage_bytes));
-    const char* xh = static_cast<const char*>(x);
-    bool used[2] = {false, false};
-    int buf = 0;
-    for (int64_t o0 = 0; o0 < nouter; o0 += ko) {
-      const int64_t k = std::min(ko, nouter - o0);
-      for (int64_t c0 = 0; c0 < ninner; c0 += nb) {
-        const int64_t n = std::min(nb, ninner - c0);
-        char* in = stage[buf];
-        void* out[4] = {nullptr, nullptr, nullptr, nullptr};
-        char* op = in + b_in;
-        for (int s = 0; s < 4; ++s)
-          if (out_host[s]) {
-            out[s] = op;
-            op += b_out;
-          }
-        if (used[buf])
-          WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->stage_free[buf], 0));
-        // the band's series: k * ntime rows of n cells, one strided 2-D copy
-        WB2_CUDA_TRY(cudaMemcpy2DAsync(in, size_t(n) * es,
-                                       xh + (size_t(o0) * ntime * ninner + c0) * es,
-                                       size_t(ninner) * es, size_t(n) * es, size_t(k) * ntime,
-                                       cudaMemcpyHostToDevice, ctx->copy_stream));
-        ctx->stat_h2d_bytes += k * ntime * n * int64_t(es);
-        WB2_CUDA_TRY(cudaEventRecord(ctx->stage_copied[buf], ctx->copy_stream));
-        WB2_CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->stage_copied[buf], 0));
-        WB2_TRY(tw_launch_any(ctx, dtype, in, k, ntime, n, nbin, d_start, d_count, window,
-                              skipna, out));
-        for (int s = 0; s < 4; ++s) {
-          if (!out_host[s]) continue;
-          WB2_CUDA_TRY(cudaMemcpy2DAsync(out_host[s] + (size_t(o0) * nout * ninner + c0) * es,
-                                         size_t(ninner) * es, out[s], size_t(n) * es,
-                                         size_t(n) * es, size_t(k) * nout,
-                                         cudaMemcpyDeviceToHost, ctx->stream));
-          ctx->stat_d2h_bytes += k * nout * n * int64_t(es);
+  DeviceBlock tables;
+  const int64_t* d_start;
+  const int32_t* d_count;
+  WB2_TRY(tw_upload(ctx, nbin, bin_start, bin_count, &tables, &d_start, &d_count));
+  StagePair stage;
+  WB2_TRY(stage.alloc(stage_bytes));
+  StagePipe pipe(ctx, stage.buf[0], stage.buf[1]);
+  const char* xh = static_cast<const char*>(x);
+  for (int64_t o0 = 0; o0 < nouter; o0 += ko) {
+    const int64_t k = std::min(ko, nouter - o0);
+    for (int64_t c0 = 0; c0 < ninner; c0 += nb) {
+      const int64_t n = std::min(nb, ninner - c0);
+      char* in;
+      WB2_TRY(pipe.next(&in));
+      void* out[4] = {nullptr, nullptr, nullptr, nullptr};
+      char* op = in + b_in;
+      for (int s = 0; s < 4; ++s)
+        if (out_host[s]) {
+          out[s] = op;
+          op += b_out;
         }
-        WB2_CUDA_TRY(cudaEventRecord(ctx->stage_free[buf], ctx->stream));
-        used[buf] = true;
-        buf ^= 1;
-      }
+      // the band's series: k * ntime rows of n cells, one strided 2-D copy
+      WB2_TRY(pipe.h2d_2d(in, size_t(n) * es, xh + (size_t(o0) * ntime * ninner + c0) * es,
+                          size_t(ninner) * es, size_t(n) * es, size_t(k) * ntime));
+      WB2_TRY(pipe.ready());
+      WB2_TRY(tw_launch_any(ctx, dtype, in, k, ntime, n, nbin, d_start, d_count, window, skipna,
+                            out));
+      for (int s = 0; s < 4; ++s)
+        if (out_host[s])
+          WB2_TRY(pipe.d2h_2d(out_host[s] + (size_t(o0) * nout * ninner + c0) * es,
+                              size_t(ninner) * es, out[s], size_t(n) * es, size_t(n) * es,
+                              size_t(k) * nout));
+      WB2_TRY(pipe.done());
     }
-    WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    return WB2_OK;
-  }();
-  cudaStreamSynchronize(ctx->stream);
-  cudaStreamSynchronize(ctx->copy_stream);
-  for (int i = 0; i < 2; ++i)
-    if (stage[i]) cudaFree(stage[i]);
-  if (tables) cudaFree(tables);
-  return rc;
+  }
+  return pipe.finish();
 }
 
 }  // extern "C"
