@@ -506,7 +506,12 @@ int wb2_ens_threshold_maps(wb2_ctx* ctx, const void* x, const void* t, int dtype
  * and GaussianBrierScore / GaussianIgnoranceScore / GaussianRPS (:963-1158)
  * when nthreshold > 0 (thresholds as above):
  *         out [nfield][nthreshold][nregion][8]: [0] brier [2] ignorance [3] rps part
- * Point-wise math in float64 (the reference calls scipy.stats.norm in float64). */
+ * Point-wise math: the reference calls scipy.stats.norm in float64; here z is
+ * rounded to float32 and erfcf / expf / logf / log1pf run in float32 (a few ulp
+ * relative on min(cdf, 1 - cdf)); where that tail is below 1e-7 (|z| > 5.2) it
+ * is recomputed in float64 from the float32 z and the reference's float64
+ * `1 - cdf` is replayed, so the ignorance is inf where the reference's is
+ * (tail <= 2^-54) except in a band of about z^2 * 2^-22 relative around it. */
 int wb2_gaussian_metrics(wb2_ctx* ctx, const void* mean, const void* std,
                          const void* t, int dtype, int64_t nfield,
                          const int64_t* off_mean, const int64_t* off_std,

@@ -9,8 +9,12 @@
 //
 // Gaussian entry (wb2_gaussian_metrics): GaussianCRPS / GaussianVariance
 // (:849-937) and GaussianBrierScore / IgnoranceScore / RPS (:963-1158) from a
-// (mean, std) forecast; float64 math per cell (erfc / exp / log) because the
-// reference evaluates scipy.stats.norm in float64.
+// (mean, std) forecast.  The reference evaluates scipy.stats.norm in float64;
+// here z = (thr - mean) / std is rounded to float32 and erfcf / expf / logf /
+// log1pf run in float32 on min(cdf, 1 - cdf), which they keep to a few ulp
+// relative.  Past tail < 1e-7 (|z| > 5.2) the tail is recomputed with float64
+// erfc from the float32 z and the reference's float64 `1 - cdf` is replayed,
+// so the ignorance saturates to inf where the reference's does (tail <= 2^-54).
 //
 // Thresholds are either read from a float32 field per (threshold, field)
 // (QuantileThreshold, thresholds.py:118-149) or built in the kernel from the
@@ -280,8 +284,9 @@ __global__ void __launch_bounds__(kThrThreads, 4) threshold_kernel(const ThrPara
           // float64 would make this kernel FP64-bound (measured 0.02-0.09 of
           // the HBM roofline), so the transcendental part runs in float32 --
           // always on the tail where erfcf keeps full RELATIVE accuracy -- and
-          // only the reference's `1 - cdf` rounding step is replayed in
-          // float64 (it decides when the ignorance score saturates to inf).
+          // only the far tail (below 1e-7, rare) goes back to float64, where
+          // the reference's `1 - cdf` rounding step is replayed (it decides
+          // when the ignorance score saturates to inf).
           const float mean = g_m;
           const float sd = g_s;
           if (p.nq == 0) {
@@ -319,15 +324,22 @@ __global__ void __launch_bounds__(kThrThreads, 4) threshold_kernel(const ThrPara
                 // -log(t_gt ? pe : cdf): the argument is `tail` iff t_gt == up
                 ign = (t_gt == up) ? -logf(tail) : -log1pf(-tail);
               } else {
-                // far tail (|z| > 5.2): replay the reference's float64 `1 - cdf`
-                // rounding, which decides where the ignorance saturates to inf
-                const double cdf = up ? 1.0 - double(tail) : double(tail);
+                // far tail (|z| > 5.2): the tail again in float64 -- erfcf
+                // goes subnormal at |z| ~ 13 and to 0 at |z| ~ 14, where the
+                // reference's float64 cdf is finite down to |z| ~ 38 -- and
+                // the reference's float64 `1 - cdf` rounding replayed on it:
+                // it decides where the ignorance saturates to inf.  scipy's
+                // erfc returns 0 once a^2 > 709.78 (|z| > 37.68) where CUDA's
+                // returns a subnormal; the reference's cdf is 0 there.
+                const double a = double(fabsf(zn)) * 0.70710678118654752;
+                const double tl = a * a > 709.782712893384 ? 0.0 : 0.5 * erfc(a);
+                const double cdf = up ? 1.0 - tl : tl;
                 const double pe = 1.0 - cdf;  // exceedance probability
                 const double db = pe - (t_gt ? 1.0 : 0.0);
                 const double dr = cdf - (t_lt ? 1.0 : 0.0);
                 brier = float(db * db);
                 rps = float(dr * dr);
-                ign = -logf(float(t_gt ? pe : cdf));
+                ign = float(-log(t_gt ? pe : cdf));
               }
               val[q * kThrStats + 0] = brier;  // :980
               val[q * kThrStats + 1] = 0.f;
