@@ -12,6 +12,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel climatology --steps 3
   python benchmarks/bench_kernels.py --kernel climatology_quantile --steps 2
   python benchmarks/bench_kernels.py --kernel resample --steps 5
+  python benchmarks/bench_kernels.py --kernel wind_dynamics --steps 20
 """
 import argparse
 import json
@@ -580,12 +581,54 @@ def bench_resample(args):
       h2d_pageable_GBps=h2d, frac_of_h2d=gbs / h2d)), flush=True)
 
 
+def bench_wind_dynamics(args):
+  """Device-resident 0.25-degree (time=4, level=13, 721, 1440) u, v, z:
+  divergence (8 B read + 4 B written per cell), geostrophic wind speed (4 + 4),
+  ageostrophic wind speed (12 + 4) and vertical velocity (8 + 4), next to a
+  device copy (4 + 4) of the same field measured in the same run."""
+  torch, _lib, ctx = setup()
+  from weatherbench2_b200 import _derived_wind as dw
+  card = _card()
+  nouter, nlev = 4, 13
+  lat = np.linspace(-90, 90, NLAT)
+  lon = np.arange(NLON) * 0.25
+  lat_tab, lat_uni = dw.gradient_table(lat)
+  lon_tab, lon_uni = dw.gradient_table(lon)
+  cos = np.cos(np.deg2rad(lat))
+  cor = dw.coriolis_parameter(lat)
+  pres = 100.0 * np.array([50, 100, 150, 200, 250, 300, 400, 500, 600, 700,
+                           850, 925, 1000])
+  shape = (nouter, nlev, NLAT, NLON)
+  gen = torch.Generator(device='cuda').manual_seed(0)
+  u = torch.empty(shape, device='cuda').normal_(0, 10, generator=gen)
+  v = torch.empty(shape, device='cuda').normal_(0, 10, generator=gen)
+  z = torch.empty(shape, device='cuda').normal_(5e4, 300, generator=gen)
+  out = torch.empty(shape, device='cuda')
+  ncell = u.numel()
+  cases = [('divergence', dw.DIVERGENCE, 8),
+           ('geostrophic_wind_speed', dw.GEOSTROPHIC_WIND_SPEED, 4),
+           ('ageostrophic_wind_speed', dw.AGEOSTROPHIC_WIND_SPEED, 12),
+           ('vertical_velocity', dw.VERTICAL_VELOCITY, 8)]
+  for name, kind, read in cases:
+    fn = lambda kind=kind: ctx.wind_dynamics(
+        kind, u.data_ptr(), v.data_ptr(), z.data_ptr(), nouter, nlev, NLAT,
+        NLON, NLON, 1, lat_tab, lat_uni, lon_tab, lon_uni, cos, cor, pres,
+        out.data_ptr())
+    ms = timeit(fn, args.steps)
+    report(f'wind_dynamics {name} 4x13x721x1440', ms, ncell * (read + 4),
+           ncell, 'cells', dict(card))
+  ms = timeit(lambda: out.copy_(u), args.steps)
+  report('device copy 4x13x721x1440 (torch copy_)', ms, ncell * 8, ncell,
+         'cells', dict(card))
+
+
 if __name__ == '__main__':
   ap = argparse.ArgumentParser()
   ap.add_argument('--kernel', required=True,
                   choices=['ens', 'energy', 'det', 'regrid', 'spectrum',
                            'maps', 'threshold', 'climatology',
-                           'climatology_quantile', 'resample'])
+                           'climatology_quantile', 'resample',
+                           'wind_dynamics'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -595,4 +638,5 @@ if __name__ == '__main__':
    'threshold': bench_threshold,
    'climatology': bench_climatology,
    'climatology_quantile': bench_climatology_quantile,
-   'resample': bench_resample}[a.kernel](a)
+   'resample': bench_resample,
+   'wind_dynamics': bench_wind_dynamics}[a.kernel](a)

@@ -283,6 +283,53 @@ int wb2_seeps_maps(wb2_ctx* ctx, const float* f, const float* t, const float* we
 int wb2_wind_speed(wb2_ctx* ctx, const float* u, const float* v, float* out,
                    int64_t n);
 
+/* wb2_wind_dynamics replaces the horizontal-derivative variables of
+ * derived_variables.py:102-338 -- _d_dx / _d_dy (:102-130) and the compute() of
+ * WindDivergence, WindVorticity, VerticalVelocity (:149-209) and the geostrophic
+ * and ageostrophic winds (:231-338) -- one `kind` per output:            */
+#define WB2_DYN_DIVERGENCE 0              /* _d_dx(u) + _d_dy(v)                    */
+#define WB2_DYN_VORTICITY 1               /* _d_dx(v) - _d_dy(u)                    */
+#define WB2_DYN_VERTICAL_VELOCITY 2       /* cumulative_trapezoid(-div, 100*level)  */
+#define WB2_DYN_GEOSTROPHIC_WIND_SPEED 3  /* sqrt(ug^2 + vg^2)                      */
+#define WB2_DYN_U_GEOSTROPHIC 4           /* ug = -_d_dy(z) / f                     */
+#define WB2_DYN_V_GEOSTROPHIC 5           /* vg = _d_dx(z) / f                      */
+#define WB2_DYN_AGEOSTROPHIC_WIND_SPEED 6 /* sqrt((u - ug)^2 + (v - vg)^2)          */
+#define WB2_DYN_U_AGEOSTROPHIC 7          /* u - ug                                 */
+#define WB2_DYN_V_AGEOSTROPHIC 8          /* v - vg                                 */
+/* u, v, z   device float32 [nouter][nlev][field]; a field is nlat x nlon cells
+ *           with element strides lat_stride / lon_stride, which must be
+ *           (nlon, 1) -- (latitude, longitude) -- or (1, nlat) -- (longitude,
+ *           latitude).  Kinds 0-2 read u and v, kinds 3-5 z, kind 6 u, v and
+ *           z, kind 7 u and z, kind 8 v and z; an operand a kind does not read
+ *           may be NULL.
+ *   lat_coef, lon_coef  host [n][3] float64: np.gradient's coefficients per
+ *           index -- index 0 and n-1: the edge spacing dx[0] / dx[n-2];
+ *           interior with *_uniform != 0: 2*dx; otherwise np.gradient's a, b, c
+ *           for f[i-1], f[i], f[i+1] (the spacing is uniform when every diff of
+ *           the coordinate equals the first exactly, as np.gradient decides);
+ *   cos_lat   host [nlat] float64 cos(deg2rad(lat));
+ *   coriolis  host [nlat] float64 2 * 7.292e-5 * sin(deg2rad(lat)) (kinds 3-8);
+ *   pressure  host [nlev] float64 100 * level, in storage order (kind 2);
+ *   out       device float32, same shape and layout as the inputs.
+ * Kinds 0, 1, 3-8 treat the nouter * nlev fields alike; kind 2 walks the nlev
+ * levels of each column in one thread and integrates the float64 divergence.
+ * Numerics: for float32 data on float64 coordinates every output is the
+ * reference's float64 arithmetic (np.gradient with edge_order=1, no longitude
+ * wrap-around; _d_dx as two float64 divisions, 0 where cos(lat) <= 1e-6;
+ * _d_dy a float32 division by float32(M), M = 2 pi 6367500 / 360) rounded once
+ * to float32, bit for bit, including NaN and +-inf (the geostrophic wind is
+ * +-inf or NaN where f = 0).  Deviations: float64 data is cast to float32 by the
+ * caller first (the reference's _d_dy would then run in float64), and float32
+ * coordinates are taken as float64.  Errors: NULL operands, negative sizes, an
+ * unknown kind, nlat or nlon < 2, other strides.                              */
+int wb2_wind_dynamics(wb2_ctx* ctx, int kind, const float* u, const float* v,
+                      const float* z, int64_t nouter, int32_t nlev, int32_t nlat,
+                      int32_t nlon, int64_t lat_stride, int64_t lon_stride,
+                      const double* lat_coef, int lat_uniform,
+                      const double* lon_coef, int lon_uniform,
+                      const double* cos_lat, const double* coriolis,
+                      const double* pressure, float* out);
+
 /* wb2_ens_mean replaces the ensemble-mean pipeline of
  * scripts/compute_ensemble_mean.py:110-141 (xbeam.Mean(realization, skipna)):
  * out[field][cell] = mean_m x[off_x[field] + m * member_stride + cell], float32;

@@ -122,6 +122,11 @@ PROTOTYPES = {
                                           C.c_int64, C.POINTER(Csr),
                                           C.POINTER(Csr)]),
     'wb2_wind_speed': (C.c_int, [_P, _P, _P, _P, C.c_int64]),
+    'wb2_wind_dynamics': (C.c_int, [
+        _P, C.c_int, _P, _P, _P, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+        C.c_int64, C.c_int64, C.POINTER(C.c_double), C.c_int,
+        C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_double),
+        C.POINTER(C.c_double), C.POINTER(C.c_double), _P]),
     'wb2_ens_mean': (C.c_int, [_P, _P, C.c_int32, C.c_int64, C.c_int64, _I64P,
                                C.c_int64, C.c_int, _P]),
     'wb2_spectrum_interp': (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32,
@@ -600,6 +605,28 @@ class Context:
   # -- derived variables -------------------------------------------------------
   def wind_speed(self, u: int, v: int, out: int, n: int):
     check(self.lib.wb2_wind_speed(self.handle, _P(u), _P(v), _P(out), int(n)))
+
+  def wind_dynamics(self, kind: int, u: Optional[int], v: Optional[int],
+                    z: Optional[int], nouter: int, nlev: int, nlat: int,
+                    nlon: int, lat_stride: int, lon_stride: int,
+                    lat_coef: np.ndarray, lat_uniform: bool,
+                    lon_coef: np.ndarray, lon_uniform: bool,
+                    cos_lat: np.ndarray, coriolis: Optional[np.ndarray],
+                    pressure: Optional[np.ndarray], out: int):
+    """u / v / z / out are DEVICE addresses (wb2_wind_dynamics); the tables
+    are host float64 arrays (see the header for their layout)."""
+    tabs = [None if a is None else np.ascontiguousarray(a, dtype=np.float64)
+            for a in (lat_coef, lon_coef, cos_lat, coriolis, pressure)]
+    lc, oc, cs, cor, pres = tabs
+    check(self.lib.wb2_wind_dynamics(
+        self.handle, int(kind), _P(u) if u else None, _P(v) if v else None,
+        _P(z) if z else None, int(nouter), int(nlev), int(nlat), int(nlon),
+        int(lat_stride), int(lon_stride), _as_ptr(lc, C.c_double),
+        int(bool(lat_uniform)), _as_ptr(oc, C.c_double),
+        int(bool(lon_uniform)), _as_ptr(cs, C.c_double),
+        _as_ptr(cor, C.c_double), _as_ptr(pres, C.c_double),
+        _P(out) if out else None))
+    del tabs
 
   def ens_mean(self, x: int, nmember: int, member_stride: int,
                off_x: np.ndarray, slab: int, skipna: bool, out: int):

@@ -1,8 +1,12 @@
 """Derived variables on the hot path: `ZonalEnergySpectrum` with the API of
 weatherbench2/derived_variables.py:29-56, 531-626.  The rFFT, the power
 spectrum and the circumference scaling run in csrc/spectrum.cu.
-(The other derived variables of the reference -- wind speed, vorticity, ... --
-are cheap stencils outside the scope of SURVEY.md section 8.)
+The wind variables of derived_variables.py:59-338 -- wind speed, divergence,
+vorticity, vertical velocity and the geostrophic / ageostrophic winds -- live in
+_derived_wind.py (csrc/derived.cu, csrc/wind_dynamics.cu) and are re-exported
+here.  The remaining derived variables of the reference (eddy kinetic energy,
+lapse rate, column integrals, relative humidity, precipitation accumulations)
+are not reproduced.
 """
 from __future__ import annotations
 
@@ -288,17 +292,32 @@ def interpolate_spectral_frequencies(spectrum, wavenumber_dim: str,
 
 
 # Wind variables live in _derived_wind.py (they need DerivedVariable).
-from weatherbench2_b200._derived_wind import WindSpeed  # noqa: E402  pylint: disable=wrong-import-position
+from weatherbench2_b200._derived_wind import (  # noqa: E402  pylint: disable=wrong-import-position
+    AgeostrophicWindSpeed, GeostrophicWindSpeed, UComponentOfAgeostrophicWind,
+    UComponentOfGeostrophicWind, VComponentOfAgeostrophicWind,
+    VComponentOfGeostrophicWind, VerticalVelocity, WindDivergence,
+    WindSpeed, WindVorticity, _3DWindVariable, _AgeostrophicWindVariable,
+    _GeostrophicWindVariable)
 
 # The named derived variables of weatherbench2/derived_variables.py:724-773 that
-# have a device implementation.  The remaining entries of the reference's table
-# (divergence / vorticity, geostrophic winds, lapse rate, column integrals,
-# relative humidity, precipitation accumulations) are data preparation off the
-# hot path and are not reproduced; asking for one raises KeyError here instead
-# of silently running on the host.
+# have a device implementation: wind speed and the horizontal-derivative
+# family (divergence, vorticity, vertical velocity, geostrophic and
+# ageostrophic winds).  The remaining entries of the reference's table (eddy
+# kinetic energy, lapse rate, column integrals, relative humidity,
+# precipitation accumulations) are not reproduced; asking for one raises
+# KeyError here instead of silently running on the host.
 DERIVED_VARIABLE_DICT = {
     'wind_speed': WindSpeed(u_name='u_component_of_wind',
                             v_name='v_component_of_wind'),
     '10m_wind_speed': WindSpeed(u_name='10m_u_component_of_wind',
                                 v_name='10m_v_component_of_wind'),
+    'divergence': WindDivergence(),
+    'vorticity': WindVorticity(),
+    'vertical_velocity': VerticalVelocity(),
+    'geostrophic_wind_speed': GeostrophicWindSpeed(),
+    'u_component_of_geostrophic_wind': UComponentOfGeostrophicWind(),
+    'v_component_of_geostrophic_wind': VComponentOfGeostrophicWind(),
+    'ageostrophic_wind_speed': AgeostrophicWindSpeed(),
+    'u_component_of_ageostrophic_wind': UComponentOfAgeostrophicWind(),
+    'v_component_of_ageostrophic_wind': VComponentOfAgeostrophicWind(),
 }
