@@ -142,6 +142,34 @@ struct DeviceGuard {
   }
 };
 
+// Grows a device buffer held by the context (`buf`, capacity `cap` bytes) to
+// at least `need` bytes; the contents are not kept.  Waits for the kernels
+// that may still read the old buffer before freeing it.
+template <typename T>
+int grow_buffer(wb2_ctx* ctx, T*& buf, size_t& cap, size_t need) {
+  if (cap >= need) return WB2_OK;
+  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+  if (buf) WB2_CUDA_TRY(cudaFree(buf));
+  buf = nullptr;
+  cap = 0;
+  WB2_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&buf), need));
+  cap = need;
+  return WB2_OK;
+}
+
+// Launches `kernel` on the context's stream, first raising its dynamic
+// shared-memory limit when `smem` exceeds the default 48 KB.
+template <typename... P, typename... A>
+int launch_kernel(wb2_ctx* ctx, void (*kernel)(P...), dim3 grid, int block, size_t smem,
+                  const A&... args) {
+  if (smem > 48 * 1024)
+    WB2_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      static_cast<int>(smem)));
+  kernel<<<grid, block, smem, ctx->stream>>>(args...);
+  WB2_CUDA_TRY(cudaGetLastError());
+  return WB2_OK;
+}
+
 int validate_weights(const wb2_weights* w);
 void slab_cache_destroy(wb2_ctx* ctx);  // host_stream.cu
 

@@ -21,7 +21,7 @@
 // row_w[r][row] * seg_w[r][seg] to its own float64 accumulators.  CTAs write
 // float64 partials; a second tiny kernel adds them in a fixed order
 // (deterministic, no float atomics).
-#include "common.cuh"
+#include "region_reduce.cuh"
 
 namespace wb2 {
 
@@ -276,32 +276,13 @@ det_metrics_kernel(const DetParams p) {
   for (int idx = threadIdx.x; idx < R * WB2_DET_NSTAT; idx += kThreads) {
     const int r = idx / WB2_DET_NSTAT;
     const int st = idx % WB2_DET_NSTAT;
-    // public stat -> internal slot (or -1: not produced in this mode)
-    int slot = -1;
-    if (st < 6) {
-      if (st < NSUM) slot = st;
-    } else {
-      const int j = st - 6;  // which weight sum
-      if (MODE != MODE_CLIM && j > 0) slot = -1;
-      else slot = NSUM + (j < NCNT ? j : 0);
-    }
+    const int slot = k1_slot(st, NSUM, MODE == MODE_CLIM, SKIPNA);
     double v = 0.0;
     if (slot >= 0) {
 #pragma unroll
       for (int w = 0; w < kWarps; ++w) v += red[(w * 32 + r) * NS + slot];
     }
     out[idx] = v;
-  }
-}
-
-__global__ void det_finalize_kernel(const double* __restrict__ partial,
-                                    double* __restrict__ out, int nblk, int per_field) {
-  const int64_t field = blockIdx.x;
-  for (int i = threadIdx.x; i < per_field; i += blockDim.x) {
-    const double* src = partial + field * int64_t(nblk) * per_field + i;
-    double v = 0.0;
-    for (int b = 0; b < nblk; ++b) v += src[int64_t(b) * per_field];
-    out[field * per_field + i] = v;
   }
 }
 
@@ -312,15 +293,8 @@ static int launch_mode(wb2_ctx* ctx, const DetParams& p, int64_t nfield, bool sk
   const int ns = NSUM + (skipna ? Counts<MODE, true>::NCNT : Counts<MODE, false>::NCNT);
   size_t smem = size_t(kWarps) * 32 * ns * sizeof(double) +
                 (weighted && p.col_w ? size_t(p.ncol) * sizeof(float) : 0);
-  dim3 grid(static_cast<unsigned>(nfield * p.nblk));
-  auto go = [&](auto kernel) -> int {
-    if (smem > 48 * 1024)
-      WB2_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-    kernel<<<grid, kThreads, smem, ctx->stream>>>(p);
-    WB2_CUDA_TRY(cudaGetLastError());
-    return WB2_OK;
-  };
+  const dim3 grid(static_cast<unsigned>(nfield * p.nblk));
+  auto go = [&](auto kernel) { return launch_kernel(ctx, kernel, grid, kThreads, smem, p); };
   if (skipna) {
     if (weighted) return go(det_metrics_kernel<T, VEC, MODE, true, true>);
     return go(det_metrics_kernel<T, VEC, MODE, true, false>);
@@ -347,6 +321,7 @@ static int launch_dtype(wb2_ctx* ctx, const DetParams& p, int64_t nfield, int mo
   }
 }
 
+// det_tma.cu: 1 if the kernel ran, 0 if the launch is not eligible, < 0 on error
 int det_metrics_tma(wb2_ctx* ctx, bool clim, const void* f, const void* t, const void* c,
                     int64_t nfield, const int64_t* d_off_f, const int64_t* d_off_t,
                     const int64_t* d_off_c, const double* d_row_w, const double* d_seg_w,
@@ -393,26 +368,15 @@ int det_metrics_impl(wb2_ctx* ctx, int mode, const void* f, const void* t, const
 
   // rows per CTA: 4 rows per warp keeps the per-CTA epilogue negligible and
   // gives >= 20 waves on the headline shape (780 fields x 23 blocks).
-  int rows_per_block = 4 * kWarps;
-  int nblk = (w->nrow + rows_per_block - 1) / rows_per_block;
-  // small launches: use more, smaller blocks so that all SMs get work
-  while (nblk * nfield < 2 * ctx->num_sms && rows_per_block > kWarps) {
-    rows_per_block /= 2;
-    nblk = (w->nrow + rows_per_block - 1) / rows_per_block;
-  }
-
-  const int R = w->nregion;
-  const size_t per_field = size_t(R) * WB2_DET_NSTAT;
+  const BlockRows br = block_rows(w->nrow, nfield, 4 * kWarps, kWarps, 2 * ctx->num_sms);
+  const size_t per_field = size_t(w->nregion) * WB2_DET_NSTAT;
   Packer pk(ctx);
   size_t o_f = pk.add(off_f, nfield * sizeof(int64_t));
   size_t o_t = pk.add(off_t, nfield * sizeof(int64_t));
   size_t o_c = off_c ? pk.add(off_c, nfield * sizeof(int64_t)) : 0;
   size_t o_g = off_g ? pk.add(off_g, nfield * sizeof(int64_t)) : 0;
-  size_t o_rw = pk.add(w->row_w, size_t(R) * w->nrow * sizeof(double));
-  size_t o_ss = pk.add(w->seg_start, size_t(w->nseg + 1) * sizeof(int32_t));
-  size_t o_sw = pk.add(w->seg_w, size_t(R) * w->nseg * sizeof(double));
-  size_t o_cw = w->col_w ? pk.add(w->col_w, size_t(w->ncol) * sizeof(float)) : 0;
-  size_t o_part = pk.reserve(size_t(nfield) * nblk * per_field * sizeof(double));
+  const WeightUpload wu(pk, w);
+  size_t o_part = pk.reserve(size_t(nfield) * br.nblk * per_field * sizeof(double));
   WB2_TRY(pk.commit());
 
   DetParams p;
@@ -421,44 +385,30 @@ int det_metrics_impl(wb2_ctx* ctx, int mode, const void* f, const void* t, const
   p.off_t = pk.dev<int64_t>(o_t);
   p.off_c = off_c ? pk.dev<int64_t>(o_c) : nullptr;
   p.off_g = off_g ? pk.dev<int64_t>(o_g) : nullptr;
-  p.row_w = pk.dev<double>(o_rw);
-  p.seg_start = pk.dev<int32_t>(o_ss);
-  p.seg_w = pk.dev<double>(o_sw);
-  p.col_w = w->col_w ? pk.dev<float>(o_cw) : nullptr;
-  p.cell_w = w->cell_w;
+  wu.bind(p);
   p.partial = pk.dev<double>(o_part);
-  p.nrow = w->nrow; p.ncol = w->ncol; p.row_stride = w->row_stride;
-  p.nregion = R; p.nseg = w->nseg; p.zero_skip = w->zero_skip;
-  p.rows_per_block = rows_per_block; p.nblk = nblk;
+  p.rows_per_block = br.rows_per_block; p.nblk = br.nblk;
 
   const bool weighted = w->col_w != nullptr || w->cell_w != nullptr;
 
-  // Fast path: TMA-staged persistent kernel (det_tma.cu) when every slab is
-  // 16-byte aligned and the weights are separable with one column segment.
+  // Fast path: TMA-staged persistent kernels (det_tma.cu) when every slab is
+  // 16-byte aligned and the weights are separable: one column segment, or
+  // several (lane-contiguous column spans, for many regions).
   // WB2_DET_PATH=ldg forces the LDG kernel (A/B measurements, tests).
-  {
-    const char* force = getenv("WB2_DET_PATH");
-    const bool want_tma = !(force && strcmp(force, "ldg") == 0);
-    if (want_tma && dtype == WB2_F32 && vec_ok && !weighted && w->nseg == 1 &&
-        w->ncol % 4 == 0 && mode != MODE_VECTOR) {
-      int trc = det_metrics_tma(ctx, mode == MODE_CLIM, f, t, c, nfield, p.off_f, p.off_t,
-                                p.off_c, p.row_w, p.seg_w, w, skipna, out);
-      if (trc < 0) return trc;
-      if (trc == 1) {
-        WB2_TRY(pk.release());
-        return WB2_OK;
-      }
-    }
-    // many regions: column segments -> lane-contiguous TMA kernel
-    if (want_tma && dtype == WB2_F32 && vec_ok && !weighted && w->nseg > 1 &&
-        w->ncol % 4 == 0 && mode != MODE_VECTOR) {
-      int trc = det_metrics_tma_seg(ctx, mode == MODE_CLIM, f, t, c, nfield, p.off_f, p.off_t,
-                                    p.off_c, w, skipna, out);
-      if (trc < 0) return trc;
-      if (trc == 1) {
-        WB2_TRY(pk.release());
-        return WB2_OK;
-      }
+  const char* force = getenv("WB2_DET_PATH");
+  const bool want_tma = !(force && strcmp(force, "ldg") == 0);
+  if (want_tma && dtype == WB2_F32 && vec_ok && !weighted && w->ncol % 4 == 0 &&
+      mode != MODE_VECTOR) {
+    const int trc =
+        w->nseg == 1
+            ? det_metrics_tma(ctx, mode == MODE_CLIM, f, t, c, nfield, p.off_f, p.off_t,
+                              p.off_c, p.row_w, p.seg_w, w, skipna, out)
+            : det_metrics_tma_seg(ctx, mode == MODE_CLIM, f, t, c, nfield, p.off_f, p.off_t,
+                                  p.off_c, w, skipna, out);
+    if (trc < 0) return trc;
+    if (trc == 1) {
+      WB2_TRY(pk.release());
+      return WB2_OK;
     }
   }
 
@@ -466,9 +416,7 @@ int det_metrics_impl(wb2_ctx* ctx, int mode, const void* f, const void* t, const
                ? launch_dtype<float>(ctx, p, nfield, mode, skipna != 0, weighted, vec_ok)
                : launch_dtype<double>(ctx, p, nfield, mode, skipna != 0, weighted, vec_ok);
   if (rc != WB2_OK) return rc;
-  det_finalize_kernel<<<static_cast<unsigned>(nfield), 128, 0, ctx->stream>>>(
-      p.partial, out, nblk, static_cast<int>(per_field));
-  WB2_CUDA_TRY(cudaGetLastError());
+  WB2_TRY(launch_block_sum(ctx, p.partial, out, nfield, br.nblk, static_cast<int>(per_field)));
   ctx->launches += 2;
   WB2_TRY(pk.release());
   return WB2_OK;

@@ -10,7 +10,7 @@
 // with a smaller index -- exactly np.argsort's stable order used at
 // metrics.py:836-846, NaN last), O(M^2 / 32) per lane.  Correctness first: this
 // path is for small grids; K2 is the fast path.
-#include "common.cuh"
+#include "region_reduce.cuh"
 
 namespace wb2 {
 
@@ -147,17 +147,6 @@ __global__ void __launch_bounds__(kBigThreads) ens_big_kernel(const BigParams p)
   }
 }
 
-__global__ void ens_big_finalize_kernel(const double* __restrict__ partial,
-                                        double* __restrict__ out, int nblk, int per_field) {
-  const int64_t field = blockIdx.x;
-  for (int i = threadIdx.x; i < per_field; i += blockDim.x) {
-    const double* src = partial + field * int64_t(nblk) * per_field + i;
-    double v = 0.0;
-    for (int b = 0; b < nblk; ++b) v += src[int64_t(b) * per_field];
-    out[field * per_field + i] = v;
-  }
-}
-
 int ens_metrics_big(wb2_ctx* ctx, const float* x, const float* t, int32_t nmember,
                     int64_t member_stride, int64_t nfield, const int64_t* off_x,
                     const int64_t* off_t, const wb2_weights* w, int skipna, double* out) {
@@ -178,32 +167,20 @@ int ens_metrics_big(wb2_ctx* ctx, const float* x, const float* t, int32_t nmembe
   Packer pk(ctx);
   size_t o_x = pk.add(off_x, nfield * sizeof(int64_t));
   size_t o_t = pk.add(off_t, nfield * sizeof(int64_t));
-  size_t o_rw = pk.add(w->row_w, size_t(R) * w->nrow * sizeof(double));
-  size_t o_ss = pk.add(w->seg_start, size_t(w->nseg + 1) * sizeof(int32_t));
-  size_t o_sw = pk.add(w->seg_w, size_t(R) * w->nseg * sizeof(double));
-  size_t o_cw = w->col_w ? pk.add(w->col_w, size_t(w->ncol) * sizeof(float)) : 0;
+  const WeightUpload wu(pk, w);
   size_t o_part = pk.reserve(size_t(nfield) * nblk * per_field * sizeof(double));
   WB2_TRY(pk.commit());
   BigParams p;
   p.x = x; p.t = t;
   p.off_x = pk.dev<int64_t>(o_x); p.off_t = pk.dev<int64_t>(o_t);
-  p.row_w = pk.dev<double>(o_rw); p.seg_start = pk.dev<int32_t>(o_ss);
-  p.seg_w = pk.dev<double>(o_sw);
-  p.col_w = w->col_w ? pk.dev<float>(o_cw) : nullptr;
-  p.cell_w = w->cell_w;
+  wu.bind(p);
   p.partial = pk.dev<double>(o_part);
-  p.member_stride = member_stride; p.row_stride = w->row_stride;
-  p.nmember = nmember; p.nrow = w->nrow; p.ncol = w->ncol;
-  p.nregion = R; p.nseg = w->nseg; p.zero_skip = w->zero_skip;
+  p.member_stride = member_stride;
+  p.nmember = nmember;
   p.nblk = nblk; p.tiles_per_row = tiles_per_row; p.skipna = skipna ? 1 : 0;
-  if (smem > 48 * 1024)
-    WB2_CUDA_TRY(cudaFuncSetAttribute(ens_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      static_cast<int>(smem)));
-  ens_big_kernel<<<static_cast<unsigned>(nfield * nblk), kBigThreads, smem, ctx->stream>>>(p);
-  WB2_CUDA_TRY(cudaGetLastError());
-  ens_big_finalize_kernel<<<static_cast<unsigned>(nfield), 128, 0, ctx->stream>>>(
-      p.partial, out, nblk, static_cast<int>(per_field));
-  WB2_CUDA_TRY(cudaGetLastError());
+  WB2_TRY(launch_kernel(ctx, ens_big_kernel, dim3(static_cast<unsigned>(nfield * nblk)),
+                        kBigThreads, smem, p));
+  WB2_TRY(launch_block_sum(ctx, p.partial, out, nfield, nblk, static_cast<int>(per_field)));
   ctx->launches += 2;
   WB2_TRY(pk.release());
   return WB2_OK;

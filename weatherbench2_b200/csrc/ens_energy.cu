@@ -17,7 +17,7 @@
 // K1 on member views).
 #include <algorithm>
 
-#include "common.cuh"
+#include "region_reduce.cuh"
 
 namespace wb2 {
 
@@ -204,21 +204,15 @@ extern "C" int wb2_energy_score(wb2_ctx* ctx, const void* x, const void* t, int 
   const int ngroups = (nmember + gs - 1) / gs;  // <= 8
   const int rows_in_flight = std::max(1, 8 / ngroups);
   const int warps = ngroups * rows_in_flight;
-  int rows_per_block = 8 * rows_in_flight;
-  int nblk = (w->nrow + rows_per_block - 1) / rows_per_block;
-  while (nblk * nfield < 4 * ctx->num_sms && rows_per_block > rows_in_flight) {
-    rows_per_block = std::max(rows_in_flight, rows_per_block / 2);
-    nblk = (w->nrow + rows_per_block - 1) / rows_per_block;
-  }
+  const BlockRows br =
+      block_rows(w->nrow, nfield, 8 * rows_in_flight, rows_in_flight, 4 * ctx->num_sms);
+  const int nblk = br.nblk;
   const int R = w->nregion;
   const int nacc = 2 * gs + 1;
   Packer pk(ctx);
   size_t o_x = pk.add(off_x, nfield * sizeof(int64_t));
   size_t o_t = pk.add(off_t, nfield * sizeof(int64_t));
-  size_t o_rw = pk.add(w->row_w, size_t(R) * w->nrow * sizeof(double));
-  size_t o_ss = pk.add(w->seg_start, size_t(w->nseg + 1) * sizeof(int32_t));
-  size_t o_sw = pk.add(w->seg_w, size_t(R) * w->nseg * sizeof(double));
-  size_t o_cw = w->col_w ? pk.add(w->col_w, size_t(w->ncol) * sizeof(float)) : 0;
+  const WeightUpload wu(pk, w);
   size_t o_part = pk.reserve(size_t(nfield) * nblk * rows_in_flight * ngroups * R * nacc *
                              sizeof(double));
   WB2_TRY(pk.commit());
@@ -226,15 +220,11 @@ extern "C" int wb2_energy_score(wb2_ctx* ctx, const void* x, const void* t, int 
   p.x = static_cast<const float*>(x);
   p.t = static_cast<const float*>(t);
   p.off_x = pk.dev<int64_t>(o_x); p.off_t = pk.dev<int64_t>(o_t);
-  p.row_w = pk.dev<double>(o_rw); p.seg_start = pk.dev<int32_t>(o_ss);
-  p.seg_w = pk.dev<double>(o_sw);
-  p.col_w = w->col_w ? pk.dev<float>(o_cw) : nullptr;
-  p.cell_w = w->cell_w;
+  wu.bind(p);
   p.partial = pk.dev<double>(o_part);
-  p.member_stride = member_stride; p.row_stride = w->row_stride;
-  p.nmember = nmember; p.nrow = w->nrow; p.ncol = w->ncol;
-  p.nregion = R; p.nseg = w->nseg; p.zero_skip = w->zero_skip;
-  p.rows_per_block = rows_per_block; p.nblk = nblk;
+  p.member_stride = member_stride;
+  p.nmember = nmember;
+  p.rows_per_block = br.rows_per_block; p.nblk = nblk;
   p.ngroups = ngroups; p.rows_in_flight = rows_in_flight;
   {
     bool ok = (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
@@ -245,21 +235,8 @@ extern "C" int wb2_energy_score(wb2_ctx* ctx, const void* x, const void* t, int 
     p.vec4 = ok ? 1 : 0;
   }
   const size_t smem = w->col_w ? size_t(w->ncol) * sizeof(float) : 0;
-  const unsigned grid = static_cast<unsigned>(nfield * nblk);
-  if (gs == 4) {
-    if (smem > 48 * 1024)
-      WB2_CUDA_TRY(cudaFuncSetAttribute(energy_kernel<4>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-    energy_kernel<4><<<grid, 32 * warps, smem, ctx->stream>>>(p);
-  } else {
-    if (smem > 48 * 1024)
-      WB2_CUDA_TRY(cudaFuncSetAttribute(energy_kernel<8>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-    energy_kernel<8><<<grid, 32 * warps, smem, ctx->stream>>>(p);
-  }
-  WB2_CUDA_TRY(cudaGetLastError());
+  WB2_TRY(launch_kernel(ctx, gs == 4 ? energy_kernel<4> : energy_kernel<8>,
+                        dim3(static_cast<unsigned>(nfield * nblk)), 32 * warps, smem, p));
   energy_finalize_kernel<<<static_cast<unsigned>(nfield), 128, 0, ctx->stream>>>(
       p.partial, out, nblk, rows_in_flight, ngroups, R, gs, nmember);
   WB2_CUDA_TRY(cudaGetLastError());

@@ -19,7 +19,7 @@
 // ALU-pipe / HBM ridge (see DESIGN.md).
 #include <cmath>
 
-#include "common.cuh"
+#include "region_reduce.cuh"
 #include "ens_point.cuh"
 
 namespace wb2 {
@@ -294,17 +294,6 @@ static int try_pair(wb2_ctx* ctx, const EnsParams& p, int64_t nfield, bool skipn
   }
 }
 
-__global__ void ens_finalize_kernel(const double* __restrict__ partial, double* __restrict__ out,
-                                    int nblk, int per_field) {
-  const int64_t field = blockIdx.x;
-  for (int i = threadIdx.x; i < per_field; i += blockDim.x) {
-    const double* src = partial + field * int64_t(nblk) * per_field + i;
-    double v = 0.0;
-    for (int b = 0; b < nblk; ++b) v += src[int64_t(b) * per_field];
-    out[field * per_field + i] = v;
-  }
-}
-
 template <int MP>
 static int launch_ens(wb2_ctx* ctx, const EnsParams& p, int64_t nfield, bool skipna,
                       bool aligned8) {
@@ -316,15 +305,8 @@ static int launch_ens(wb2_ctx* ctx, const EnsParams& p, int64_t nfield, bool ski
   const int ns = kEnsStats + (skipna ? kEnsStats : 1);
   const size_t smem = size_t(kEnsWarps) * 32 * ns * sizeof(double) +
                       (p.col_w ? size_t(p.ncol) * sizeof(float) : 0);
-  dim3 grid(static_cast<unsigned>(nfield * p.nblk));
-  auto go = [&](auto kernel) -> int {
-    if (smem > 48 * 1024)
-      WB2_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-    kernel<<<grid, kEnsThreads, smem, ctx->stream>>>(p);
-    WB2_CUDA_TRY(cudaGetLastError());
-    return WB2_OK;
-  };
+  const dim3 grid(static_cast<unsigned>(nfield * p.nblk));
+  auto go = [&](auto kernel) { return launch_kernel(ctx, kernel, grid, kEnsThreads, smem, p); };
   // resident CTAs per SM the register allocation targets (tuning knob)
   const char* occ_env = getenv("WB2_ENS_OCC");
   const int occ = occ_env ? atoi(occ_env) : (skipna ? 4 : 5);
@@ -378,22 +360,13 @@ extern "C" int wb2_ens_metrics(wb2_ctx* ctx, const void* x, const void* t, int d
     return ens_metrics_big(ctx, static_cast<const float*>(x), static_cast<const float*>(t),
                            nmember, member_stride, nfield, off_x, off_t, w, skipna, out);
 
-  int rows_per_block = 2 * kEnsWarps;
-  int nblk = (w->nrow + rows_per_block - 1) / rows_per_block;
-  while (nblk * nfield < 4 * ctx->num_sms && rows_per_block > kEnsWarps) {
-    rows_per_block /= 2;
-    nblk = (w->nrow + rows_per_block - 1) / rows_per_block;
-  }
-  const int R = w->nregion;
-  const size_t per_field = size_t(R) * WB2_ENS_NSTAT;
+  const BlockRows br = block_rows(w->nrow, nfield, 2 * kEnsWarps, kEnsWarps, 4 * ctx->num_sms);
+  const size_t per_field = size_t(w->nregion) * WB2_ENS_NSTAT;
   Packer pk(ctx);
   size_t o_x = pk.add(off_x, nfield * sizeof(int64_t));
   size_t o_t = pk.add(off_t, nfield * sizeof(int64_t));
-  size_t o_rw = pk.add(w->row_w, size_t(R) * w->nrow * sizeof(double));
-  size_t o_ss = pk.add(w->seg_start, size_t(w->nseg + 1) * sizeof(int32_t));
-  size_t o_sw = pk.add(w->seg_w, size_t(R) * w->nseg * sizeof(double));
-  size_t o_cw = w->col_w ? pk.add(w->col_w, size_t(w->ncol) * sizeof(float)) : 0;
-  size_t o_part = pk.reserve(size_t(nfield) * nblk * per_field * sizeof(double));
+  const WeightUpload wu(pk, w);
+  size_t o_part = pk.reserve(size_t(nfield) * br.nblk * per_field * sizeof(double));
   WB2_TRY(pk.commit());
 
   EnsParams p;
@@ -401,18 +374,11 @@ extern "C" int wb2_ens_metrics(wb2_ctx* ctx, const void* x, const void* t, int d
   p.t = static_cast<const float*>(t);
   p.off_x = pk.dev<int64_t>(o_x);
   p.off_t = pk.dev<int64_t>(o_t);
-  p.row_w = pk.dev<double>(o_rw);
-  p.seg_start = pk.dev<int32_t>(o_ss);
-  p.seg_w = pk.dev<double>(o_sw);
-  p.col_w = w->col_w ? pk.dev<float>(o_cw) : nullptr;
-  p.cell_w = w->cell_w;
+  wu.bind(p);
   p.partial = pk.dev<double>(o_part);
   p.member_stride = member_stride;
-  p.row_stride = w->row_stride;
   p.nmember = nmember;
-  p.nrow = w->nrow; p.ncol = w->ncol;
-  p.nregion = R; p.nseg = w->nseg; p.zero_skip = w->zero_skip;
-  p.rows_per_block = rows_per_block; p.nblk = nblk;
+  p.rows_per_block = br.rows_per_block; p.nblk = br.nblk;
 
   int rc;
   const bool sk = skipna != 0;
@@ -433,9 +399,7 @@ extern "C" int wb2_ens_metrics(wb2_ctx* ctx, const void* x, const void* t, int d
   else if (nmember <= 50) rc = launch_ens<50>(ctx, p, nfield, sk, aligned8);
   else rc = launch_ens<64>(ctx, p, nfield, sk, aligned8);
   if (rc != WB2_OK) return rc;
-  ens_finalize_kernel<<<static_cast<unsigned>(nfield), 128, 0, ctx->stream>>>(
-      p.partial, out, nblk, static_cast<int>(per_field));
-  WB2_CUDA_TRY(cudaGetLastError());
+  WB2_TRY(launch_block_sum(ctx, p.partial, out, nfield, br.nblk, static_cast<int>(per_field)));
   ctx->launches += 2;
   WB2_TRY(pk.release());
   return WB2_OK;

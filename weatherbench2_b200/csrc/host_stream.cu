@@ -62,17 +62,6 @@ static int ensure_stage(wb2_ctx* ctx, size_t need) {
   return WB2_OK;
 }
 
-static int ensure_out_tmp(wb2_ctx* ctx, size_t need) {
-  if (ctx->out_tmp_cap >= need) return WB2_OK;
-  WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-  if (ctx->d_out_tmp) WB2_CUDA_TRY(cudaFree(ctx->d_out_tmp));
-  ctx->d_out_tmp = nullptr;
-  ctx->out_tmp_cap = 0;
-  WB2_CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&ctx->d_out_tmp), need));
-  ctx->out_tmp_cap = need;
-  return WB2_OK;
-}
-
 void slab_cache_destroy(wb2_ctx* ctx) {
   SlabCache* c = static_cast<SlabCache*>(ctx->slab_cache);
   if (!c) return;
@@ -219,7 +208,8 @@ int wb2_det_metrics_host(wb2_ctx* ctx, const void* f, const void* t, const void*
   WB2_TRY(ensure_stage(ctx, cap));
   const int64_t max_slabs = int64_t(ctx->stage_cap / slab_bytes);
   const size_t per_field = size_t(w->nregion) * WB2_DET_NSTAT;
-  WB2_TRY(ensure_out_tmp(ctx, size_t(nfield) * per_field * sizeof(double)));
+  WB2_TRY(grow_buffer(ctx, ctx->d_out_tmp, ctx->out_tmp_cap,
+                      size_t(nfield) * per_field * sizeof(double)));
   int crc;
   SlabCache* cache = cache_for(ctx, slab_bytes, &crc);
   if (crc != WB2_OK) return crc;
@@ -324,7 +314,8 @@ int wb2_ens_metrics_host(wb2_ctx* ctx, const void* x, const void* t, int dtype,
   WB2_TRY(ensure_stage(ctx, cap));
   const int64_t fields_per_group = std::max<int64_t>(1, int64_t(ctx->stage_cap / slab_bytes) / per);
   const size_t per_field = size_t(w->nregion) * WB2_ENS_NSTAT;
-  WB2_TRY(ensure_out_tmp(ctx, size_t(nfield) * per_field * sizeof(double)));
+  WB2_TRY(grow_buffer(ctx, ctx->d_out_tmp, ctx->out_tmp_cap,
+                      size_t(nfield) * per_field * sizeof(double)));
   int crc;
   SlabCache* cache = cache_for(ctx, slab_bytes, &crc);
   if (crc != WB2_OK) return crc;
@@ -481,7 +472,7 @@ static int spectrum_host(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t n
   const int64_t k = std::max<int64_t>(1, fit / S);
   const size_t acc_bytes = size_t(nfield_out) * out_elems * 4;
   // the device accumulator lives in out_tmp (scratch is used by the kernels)
-  WB2_TRY(ensure_out_tmp(ctx, acc_bytes));
+  WB2_TRY(grow_buffer(ctx, ctx->d_out_tmp, ctx->out_tmp_cap, acc_bytes));
   float* acc = reinterpret_cast<float*>(ctx->d_out_tmp);
   WB2_CUDA_TRY(cudaMemsetAsync(acc, 0, acc_bytes, ctx->stream));
   StagePipe pipe(ctx, ctx->stage[0], ctx->stage[1]);

@@ -512,14 +512,7 @@ int spectrum_latsum_impl(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t n
   // scratch, then the row sum
   const int nk = ncol / 2 + 1;
   const size_t need = size_t(nfield_out) * nrow * nk * sizeof(float);
-  if (need > ctx->scratch_cap) {
-    WB2_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
-    if (ctx->scratch) WB2_CUDA_TRY(cudaFree(ctx->scratch));
-    ctx->scratch = nullptr;
-    ctx->scratch_cap = 0;
-    WB2_CUDA_TRY(cudaMalloc(&ctx->scratch, need));
-    ctx->scratch_cap = need;
-  }
+  WB2_TRY(grow_buffer(ctx, ctx->scratch, ctx->scratch_cap, need));
   float* spec = static_cast<float*>(ctx->scratch);
   WB2_CUDA_TRY(cudaMemsetAsync(spec, 0, need, ctx->stream));
   WB2_TRY(wb2_zonal_spectrum(ctx, x, nfield, nrow, ncol, scale, spec, 1, nfield_out));

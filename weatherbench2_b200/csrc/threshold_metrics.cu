@@ -24,7 +24,7 @@
 //   x > thr  <=>  x > round_down_f32(thr),   x < thr  <=>  x < round_up_f32(thr).
 #include <cmath>
 
-#include "common.cuh"
+#include "region_reduce.cuh"
 
 namespace wb2 {
 
@@ -386,30 +386,12 @@ __global__ void __launch_bounds__(kThrThreads, 4) threshold_kernel(const ThrPara
   }
 }
 
-__global__ void threshold_finalize_kernel(const double* __restrict__ partial,
-                                          double* __restrict__ out, int nblk, int per_field) {
-  const int64_t field = blockIdx.x;
-  for (int i = threadIdx.x; i < per_field; i += blockDim.x) {
-    const double* src = partial + field * int64_t(nblk) * per_field + i;
-    double v = 0.0;
-    for (int b = 0; b < nblk; ++b) v += src[int64_t(b) * per_field];
-    out[field * per_field + i] = v;
-  }
-}
-
 template <int TQ, bool GAUSS>
 static int launch_threshold(wb2_ctx* ctx, const ThrParams& p, int64_t nfield, bool skipna) {
   const size_t smem = size_t(kThrWarps) * 32 * 2 * TQ * kThrStats * sizeof(double) +
                       (p.col_w ? size_t(p.ncol) * sizeof(float) : 0);
   const dim3 grid(static_cast<unsigned>(nfield * p.nblk));
-  auto go = [&](auto kernel) -> int {
-    if (smem > 48 * 1024)
-      WB2_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        static_cast<int>(smem)));
-    kernel<<<grid, kThrThreads, smem, ctx->stream>>>(p);
-    WB2_CUDA_TRY(cudaGetLastError());
-    return WB2_OK;
-  };
+  auto go = [&](auto kernel) { return launch_kernel(ctx, kernel, grid, kThrThreads, smem, p); };
   return skipna ? go(threshold_kernel<TQ, true, GAUSS>) : go(threshold_kernel<TQ, false, GAUSS>);
 }
 
@@ -420,15 +402,9 @@ static int threshold_impl(wb2_ctx* ctx, bool gauss, const float* x, const float*
                           const int64_t* off_x, const int64_t* off_s, const int64_t* off_t,
                           const int64_t* off_a, const int64_t* off_b, const wb2_weights* w,
                           int skipna, double* out) {
-  int rows_per_block = 2 * kThrWarps;
-  int nblk = (w->nrow + rows_per_block - 1) / rows_per_block;
-  while (nblk * nfield < 4 * ctx->num_sms && rows_per_block > kThrWarps) {
-    rows_per_block /= 2;
-    nblk = (w->nrow + rows_per_block - 1) / rows_per_block;
-  }
-  const int R = w->nregion;
+  const BlockRows br = block_rows(w->nrow, nfield, 2 * kThrWarps, kThrWarps, 4 * ctx->num_sms);
   const int nq_out = nq > 0 ? nq : 1;
-  const size_t per_field = size_t(nq_out) * R * kThrOut;
+  const size_t per_field = size_t(nq_out) * w->nregion * kThrOut;
   const bool gq = thr_b != nullptr;
   Packer pk(ctx);
   const size_t o_x = pk.add(off_x, nfield * sizeof(int64_t));
@@ -437,11 +413,8 @@ static int threshold_impl(wb2_ctx* ctx, bool gauss, const float* x, const float*
   const size_t o_a = nq > 0 ? pk.add(off_a, size_t(gq ? 1 : nq) * nfield * sizeof(int64_t)) : 0;
   const size_t o_b = gq ? pk.add(off_b, nfield * sizeof(int64_t)) : 0;
   const size_t o_z = gq ? pk.add(z, size_t(nq) * sizeof(double)) : 0;
-  const size_t o_rw = pk.add(w->row_w, size_t(R) * w->nrow * sizeof(double));
-  const size_t o_ss = pk.add(w->seg_start, size_t(w->nseg + 1) * sizeof(int32_t));
-  const size_t o_sw = pk.add(w->seg_w, size_t(R) * w->nseg * sizeof(double));
-  const size_t o_cw = w->col_w ? pk.add(w->col_w, size_t(w->ncol) * sizeof(float)) : 0;
-  const size_t o_part = pk.reserve(size_t(nfield) * nblk * per_field * sizeof(double));
+  const WeightUpload wu(pk, w);
+  const size_t o_part = pk.reserve(size_t(nfield) * br.nblk * per_field * sizeof(double));
   WB2_TRY(pk.commit());
 
   ThrParams p;
@@ -452,19 +425,12 @@ static int threshold_impl(wb2_ctx* ctx, bool gauss, const float* x, const float*
   p.off_a = nq > 0 ? pk.dev<int64_t>(o_a) : nullptr;
   p.off_b = gq ? pk.dev<int64_t>(o_b) : nullptr;
   p.z = gq ? pk.dev<double>(o_z) : nullptr;
-  p.row_w = pk.dev<double>(o_rw);
-  p.seg_start = pk.dev<int32_t>(o_ss);
-  p.seg_w = pk.dev<double>(o_sw);
-  p.col_w = w->col_w ? pk.dev<float>(o_cw) : nullptr;
-  p.cell_w = w->cell_w;
+  wu.bind(p);
   p.partial = pk.dev<double>(o_part);
   p.member_stride = member_stride;
-  p.row_stride = w->row_stride;
   p.nfield = nfield;
   p.nmember = nmember;
-  p.nrow = w->nrow; p.ncol = w->ncol;
-  p.nregion = R; p.nseg = w->nseg; p.zero_skip = w->zero_skip;
-  p.rows_per_block = rows_per_block; p.nblk = nblk;
+  p.rows_per_block = br.rows_per_block; p.nblk = br.nblk;
   p.nq = nq;
   const bool sk = skipna != 0;
   int launches = 0;
@@ -484,9 +450,7 @@ static int threshold_impl(wb2_ctx* ctx, bool gauss, const float* x, const float*
     if (rc != WB2_OK) return rc;
     ++launches;
   }
-  threshold_finalize_kernel<<<static_cast<unsigned>(nfield), 128, 0, ctx->stream>>>(
-      p.partial, out, nblk, static_cast<int>(per_field));
-  WB2_CUDA_TRY(cudaGetLastError());
+  WB2_TRY(launch_block_sum(ctx, p.partial, out, nfield, br.nblk, static_cast<int>(per_field)));
   ctx->launches += launches + 1;
   WB2_TRY(pk.release());
   return WB2_OK;
