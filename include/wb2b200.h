@@ -79,7 +79,11 @@ typedef struct wb2_ctx wb2_ctx;
  * row_w (or col_w*seg_w for the latitude-fastest layout), longitude boxes in
  * seg_w (or row_w), a LandRegion mask in cell_w.
  * zero_skip != 0 reproduces `dataset.where(weights > 0, 0)` (metrics.py:160):
- * cells whose weight is zero contribute nothing, even when they hold NaN/Inf. */
+ * cells whose weight is zero contribute nothing, even when they hold NaN/Inf.
+ * It requires non-negative weights: a negative row_w / seg_w / col_w entry is
+ * rejected with WB2_EINVAL (cell_w, a device array, is not checked; it must be
+ * non-negative too).  With zero_skip == 0 any sign is accepted and the sums
+ * are linear in W.                                                          */
 typedef struct {
   int32_t nrow;            /* slow spatial axis length                         */
   int32_t ncol;            /* contiguous spatial axis length                   */

@@ -73,6 +73,20 @@ int validate_weights(const wb2_weights* w) {
   for (int k = 0; k < w->nseg; ++k)
     WB2_REQUIRE(w->seg_start[k] < w->seg_start[k + 1],
                 "weights: seg_start must be strictly increasing");
+  // The kernels skip cells whose weight == 0, the reference those whose
+  // weight is not > 0: the two agree only without negative weights.  (cell_w
+  // is a device array and is not checked here.)
+  if (w->zero_skip) {
+    for (int64_t i = 0; i < int64_t(w->nregion) * w->nrow; ++i)
+      WB2_REQUIRE(!(w->row_w[i] < 0), "weights: zero_skip needs non-negative weights "
+                  "(row_w[%lld] = %g)", static_cast<long long>(i), w->row_w[i]);
+    for (int64_t i = 0; i < int64_t(w->nregion) * w->nseg; ++i)
+      WB2_REQUIRE(!(w->seg_w[i] < 0), "weights: zero_skip needs non-negative weights "
+                  "(seg_w[%lld] = %g)", static_cast<long long>(i), w->seg_w[i]);
+    for (int i = 0; w->col_w && i < w->ncol; ++i)
+      WB2_REQUIRE(!(w->col_w[i] < 0), "weights: zero_skip needs non-negative weights "
+                  "(col_w[%d] = %g)", i, static_cast<double>(w->col_w[i]));
+  }
   return WB2_OK;
 }
 

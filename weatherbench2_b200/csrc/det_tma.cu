@@ -684,36 +684,55 @@ int det_metrics_tma_seg(wb2_ctx* ctx, bool clim, const void* f, const void* t, c
     for (size_t i = 0; i < best.size(); ++i) h_spans[half * kSegMaxSpans + i] = best[i];
   }
 
-  for (int r0 = 0; r0 < w->nregion; r0 += rch) {
-    const int nreg = std::min(rch, w->nregion - r0);
+  // The tables of every region chunk go up in ONE Packer: the caller holds a
+  // Packer slot (offset tables, weights) until this returns, and a Packer per
+  // chunk would wrap the ring of kNumSlots slots at four chunks and overwrite
+  // it while the kernels still read it.
+  const int nchunk = static_cast<int>(chunks.size());
+  std::vector<std::vector<float>> seg_wf(nchunk);
+  std::vector<size_t> o_rc(nchunk), o_rb(nchunk), o_pat(nchunk), o_sw(nchunk);
+  Packer pk(ctx);
+  for (int ci = 0; ci < nchunk; ++ci) {
+    const int r0 = ci * rch, nreg = std::min(rch, w->nregion - r0);
     // float32 weights of this region chunk
-    const ChunkBands& cb = chunks[r0 / rch];
-    std::vector<float> seg_wf(size_t(w->nseg) * rch, 0.f);
+    seg_wf[ci].assign(size_t(w->nseg) * rch, 0.f);
     for (int r = 0; r < nreg; ++r)
       for (int k = 0; k < w->nseg; ++k)
-        seg_wf[size_t(k) * rch + r] = static_cast<float>(w->seg_w[size_t(r0 + r) * w->nseg + k]);
+        seg_wf[ci][size_t(k) * rch + r] =
+            static_cast<float>(w->seg_w[size_t(r0 + r) * w->nseg + k]);
+    const ChunkBands& cb = chunks[ci];
+    o_rc[ci] = pk.add(cb.row_c.data(), cb.row_c.size() * sizeof(float));
+    o_rb[ci] = pk.add(cb.row_band.data(), cb.row_band.size() * sizeof(int32_t));
+    o_pat[ci] = pk.add(cb.pat.data(), cb.pat.size() * sizeof(float));
+    o_sw[ci] = pk.add(seg_wf[ci].data(), seg_wf[ci].size() * sizeof(float));
+  }
+  const size_t o3 = pk.add(w->seg_start, size_t(w->nseg + 1) * sizeof(int32_t));
+  const size_t o4 = pk.add(h_spans.data(), h_spans.size() * sizeof(int4));
+  {
+    // the first chunk has the most regions
+    const size_t per_field = size_t(std::min(rch, w->nregion)) * WB2_DET_NSTAT;
+    const size_t need = size_t(ncta) * CW * maxslots * per_field * sizeof(double) +
+                        size_t(nfield) * per_field * sizeof(double);
+    WB2_TRY(grow_buffer(ctx, ctx->tma_partial, ctx->tma_partial_cap, need));
+  }
+  WB2_TRY(pk.commit());
+
+  for (int r0 = 0; r0 < w->nregion; r0 += rch) {
+    const int ci = r0 / rch;
+    const int nreg = std::min(rch, w->nregion - r0);
+    const ChunkBands& cb = chunks[ci];
     const size_t per_field = size_t(nreg) * WB2_DET_NSTAT;
     const size_t part_bytes =
         size_t(ncta) * CW * maxslots * per_field * sizeof(double);
-    const size_t tmp_bytes = size_t(nfield) * per_field * sizeof(double);
-    const size_t need = part_bytes + tmp_bytes;
-    WB2_TRY(grow_buffer(ctx, ctx->tma_partial, ctx->tma_partial_cap, need));
-    Packer pk(ctx);
-    size_t o1 = pk.add(cb.row_c.data(), cb.row_c.size() * sizeof(float));
-    size_t o5 = pk.add(cb.row_band.data(), cb.row_band.size() * sizeof(int32_t));
-    size_t o6 = pk.add(cb.pat.data(), cb.pat.size() * sizeof(float));
-    size_t o2 = pk.add(seg_wf.data(), seg_wf.size() * sizeof(float));
-    size_t o3 = pk.add(w->seg_start, size_t(w->nseg + 1) * sizeof(int32_t));
-    size_t o4 = pk.add(h_spans.data(), h_spans.size() * sizeof(int4));
-    WB2_TRY(pk.commit());
 
     TmaSegParams p;
     p.f = static_cast<const float*>(f);
     p.t = static_cast<const float*>(t);
     p.c = static_cast<const float*>(c);
     p.off_f = d_off_f; p.off_t = d_off_t; p.off_c = d_off_c;
-    p.row_c = pk.dev<float>(o1); p.seg_wf = pk.dev<float>(o2);
-    p.row_band = pk.dev<int32_t>(o5); p.pat = pk.dev<float>(o6); p.nband = cb.nband;
+    p.row_c = pk.dev<float>(o_rc[ci]); p.seg_wf = pk.dev<float>(o_sw[ci]);
+    p.row_band = pk.dev<int32_t>(o_rb[ci]); p.pat = pk.dev<float>(o_pat[ci]);
+    p.nband = cb.nband;
     p.seg_start = pk.dev<int32_t>(o3);
     p.spans = pk.dev<int4>(o4);
     p.nspan[0] = h_nspan[0]; p.nspan[1] = h_nspan[1];
@@ -742,8 +761,8 @@ int det_metrics_tma_seg(wb2_ctx* ctx, bool clim, const void* f, const void* t, c
       WB2_CUDA_TRY(cudaGetLastError());
       ctx->launches += 1;
     }
-    WB2_TRY(pk.release());
   }
+  WB2_TRY(pk.release());
   return 1;
 }
 
