@@ -13,6 +13,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel climatology_quantile --steps 2
   python benchmarks/bench_kernels.py --kernel resample --steps 5
   python benchmarks/bench_kernels.py --kernel wind_dynamics --steps 20
+  python benchmarks/bench_kernels.py --kernel precip_accumulation --steps 20
 """
 import argparse
 import json
@@ -622,13 +623,77 @@ def bench_wind_dynamics(args):
          'cells', dict(card))
 
 
+def precip_bytes(nouter, ntime, ninner, window, esize=4, block=256):
+  """Bytes a precipitation accumulation needs: the input read once plus the
+  `window` halo rows each block of `block` outputs stages again, and the
+  output written once."""
+  halo = window * -(-ntime // block)
+  return (nouter * (ntime + halo) * ninner + nouter * ntime * ninner) * esize
+
+
+def bench_precip_accumulation(args):
+  """Device-resident 721 x 1440 cumulative precipitation: 2 inits x 41
+  six-hourly leads with w = 4 (24 h), 1 init x 241 hourly leads with w = 24;
+  then 2 x 41 x 181 x 360 streamed from host memory; each next to a torch
+  device copy of the same bytes measured in the same run."""
+  import time
+  torch, _lib, ctx = setup()
+  card = _card()
+  ncell = NLAT * NLON
+  gen = torch.Generator(device='cuda').manual_seed(0)
+  for nouter, ntime, window in ((2, 41, 4), (1, 241, 24)):
+    x = torch.empty((nouter, ntime, ncell), device='cuda').exponential_(
+        1e3, generator=gen).cumsum(1)
+    out = torch.empty_like(x)
+    fn = lambda: ctx.precip_accumulation(  # noqa: E731
+        x.data_ptr(), _lib.F32, nouter, ntime, ncell, window, True,
+        out.data_ptr())
+    ms = timeit(fn, args.steps)
+    report(f'precip_accumulation device {nouter}x{ntime}x721x1440 w={window}',
+           ms, precip_bytes(nouter, ntime, ncell, window), x.numel(),
+           'values', dict(card))
+    ms = timeit(lambda: out.copy_(x), args.steps)
+    report(f'device copy {nouter}x{ntime}x721x1440 (torch copy_)', ms,
+           2 * x.numel() * 4, x.numel(), 'values', dict(card))
+    del x, out
+  torch.cuda.empty_cache()
+  from weatherbench2_b200 import resampling
+  ncell = 181 * 360
+  rs = np.random.default_rng(0)
+  xh = np.cumsum(rs.exponential(1e-3, size=(2, 41, ncell)).astype(np.float32),
+                 axis=1, dtype=np.float32)
+  oh = np.empty_like(xh)
+  run = lambda: ctx.precip_accumulation_host(  # noqa: E731
+      xh.ctypes.data, _lib.F32, 2, 41, ncell, 4, True,
+      resampling.STREAM_BUDGET_BYTES, oh.ctypes.data)
+  run()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    run()
+  s = (time.perf_counter() - t0) / args.steps
+  dev = torch.empty(xh.size, device='cuda')
+  src = torch.from_numpy(xh.reshape(-1))
+  dev.copy_(src)
+  torch.cuda.synchronize()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    dev.copy_(src)
+    src.copy_(dev)
+  torch.cuda.synchronize()
+  rt = (time.perf_counter() - t0) / args.steps
+  print(json.dumps(dict(
+      card, kernel='precip_accumulation streamed 2x41x181x360 w=4',
+      ms=s * 1e3, algorithmic_GB=precip_bytes(2, 41, ncell, 4) / 1e9,
+      torch_pageable_roundtrip_ms=rt * 1e3)), flush=True)
+
+
 if __name__ == '__main__':
   ap = argparse.ArgumentParser()
   ap.add_argument('--kernel', required=True,
                   choices=['ens', 'energy', 'det', 'regrid', 'spectrum',
                            'maps', 'threshold', 'climatology',
                            'climatology_quantile', 'resample',
-                           'wind_dynamics'])
+                           'wind_dynamics', 'precip_accumulation'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -639,4 +704,5 @@ if __name__ == '__main__':
    'climatology': bench_climatology,
    'climatology_quantile': bench_climatology_quantile,
    'resample': bench_resample,
-   'wind_dynamics': bench_wind_dynamics}[a.kernel](a)
+   'wind_dynamics': bench_wind_dynamics,
+   'precip_accumulation': bench_precip_accumulation}[a.kernel](a)

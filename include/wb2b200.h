@@ -493,6 +493,33 @@ int wb2_time_window_stats_host(wb2_ctx* ctx, const void* x, int dtype, int64_t n
                                int32_t window, int skipna, size_t budget, void* mean,
                                void* min, void* max, void* sum);
 
+/* ---- precipitation accumulations over lead time -----------------------------------
+ * wb2_precip_accumulation replaces PrecipitationAccumulation.compute
+ * (weatherbench2/derived_variables.py:471-528): diff along the lead axis, a rolling
+ * sum of `window` differences, negative sums set to 0, a NaN step in front.  x is a
+ * cumulative series [nouter][ntime][ninner] (float32 or float64, read in place, so
+ * any C-contiguous array with the lead axis in the middle); out is device
+ * [nouter][ntime][ninner] of x's dtype T.  Per output step t:
+ *   t < window      NaN (every output is NaN when window >= ntime)
+ *   otherwise       d[k] = T(x[k] - x[k-1]), rounded in T as xarray's diff does;
+ *                   s = d[t-w+1] + d[t-w+2] + ... + d[t] accumulated in float64 in
+ *                   that order (oldest first), rounded once to T
+ *   clamp_negative  a rounded sum < 0 becomes +0.0; NaN stays NaN and -0.0 is kept
+ * NaN and +-Inf follow from that arithmetic: a NaN anywhere in x[t-w .. t] gives
+ * NaN, an Inf inside the window gives inf + -inf = NaN.  The reference sums float32
+ * data in float32; the gap to it is at most (w + 1) 2^-24 sum |d[k]|.  window must
+ * be >= 1 and at most 1024 unless window >= ntime.  One kernel launch per call.   */
+int wb2_precip_accumulation(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter,
+                            int64_t ntime, int64_t ninner, int32_t window,
+                            int clamp_negative, void* out);
+
+/* wb2_precip_accumulation on a HOST series (NumPy / memmap), streamed in bands like
+ * wb2_time_window_stats_host within `budget` device bytes; out is a host array of
+ * the same layout.                                                                  */
+int wb2_precip_accumulation_host(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter,
+                                 int64_t ntime, int64_t ninner, int32_t window,
+                                 int clamp_negative, size_t budget, void* out);
+
 /* ---- K10: rank histogram ---------------------------------------------------------
  * Replaces RankHistogram.compute_chunk (metrics.py:1894-2042) and the time mean
  * of EnsembleMetric.compute: rank of the truth among the members (NaN last),

@@ -195,6 +195,12 @@ PROTOTYPES = {
     'wb2_time_window_stats_host': (C.c_int, [
         _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I64P,
         _I32P, C.c_int32, C.c_int, C.c_size_t, _P, _P, _P, _P]),
+    'wb2_precip_accumulation': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int,
+        _P]),
+    'wb2_precip_accumulation_host': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int,
+        C.c_size_t, _P]),
 }
 # wb2_climatology_quantile: quantiles per call, nitem * window_size per window
 CLIM_MAX_QUANTILES = 16
@@ -742,6 +748,25 @@ class Context:
         int(window), int(bool(skipna)), int(budget),
         *(_P(p) if p else None for p in (mean, min, max, sum))))
     del keep
+
+  # -- precipitation accumulations over lead time -----------------------------
+  def precip_accumulation(self, x: int, dtype: int, nouter: int, ntime: int,
+                          ninner: int, window: int, clamp_negative: bool,
+                          out: int):
+    """x and out are DEVICE addresses (wb2_precip_accumulation)."""
+    check(self.lib.wb2_precip_accumulation(
+        self.handle, _P(x) if x else None, dtype, int(nouter), int(ntime),
+        int(ninner), int(window), int(bool(clamp_negative)),
+        _P(out) if out else None))
+
+  def precip_accumulation_host(self, x: int, dtype: int, nouter: int,
+                               ntime: int, ninner: int, window: int,
+                               clamp_negative: bool, budget: int, out: int):
+    """x and out are HOST addresses (wb2_precip_accumulation_host)."""
+    check(self.lib.wb2_precip_accumulation_host(
+        self.handle, _P(x) if x else None, dtype, int(nouter), int(ntime),
+        int(ninner), int(window), int(bool(clamp_negative)), int(budget),
+        _P(out) if out else None))
 
   # -- K10 --------------------------------------------------------------------
   def rank_histogram(self, x: int, t: int, nmember: int, member_stride: int,

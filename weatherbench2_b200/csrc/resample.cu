@@ -381,57 +381,18 @@ int wb2_time_window_stats_host(wb2_ctx* ctx, const void* x, int dtype, int64_t n
   if (nouter == 0 || ninner == 0 || nout == 0) return WB2_OK;
   WB2_REQUIRE(x != nullptr, "x is NULL");
   DeviceGuard guard(ctx->device);
-  const size_t es = dtype == WB2_F32 ? 4 : 8;
   char* const out_host[4] = {static_cast<char*>(mean), static_cast<char*>(min),
                              static_cast<char*>(max), static_cast<char*>(sum)};
-  int nstat = 0;
-  for (char* p : out_host) nstat += p != nullptr;
-
-  // bands: whole outer indices when one fits the budget, else inner cells of one
-  const size_t per_cell = (size_t(ntime) + size_t(nstat) * nout) * es;
-  const int64_t cells = std::max<int64_t>(1, static_cast<int64_t>(budget / (2 * per_cell)));
-  const int64_t nb = std::min(cells, ninner);
-  const int64_t ko = nb == ninner ? std::max<int64_t>(1, std::min(cells / ninner, nouter)) : 1;
-  auto al = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_in = al(size_t(ko) * nb * ntime * es), b_out = al(size_t(ko) * nb * nout * es);
-  const size_t stage_bytes = b_in + nstat * b_out;
-
   DeviceBlock tables;
   const int64_t* d_start;
   const int32_t* d_count;
   WB2_TRY(tw_upload(ctx, nbin, bin_start, bin_count, &tables, &d_start, &d_count));
-  StagePair stage;
-  WB2_TRY(stage.alloc(stage_bytes));
-  StagePipe pipe(ctx, stage.buf[0], stage.buf[1]);
-  const char* xh = static_cast<const char*>(x);
-  for (int64_t o0 = 0; o0 < nouter; o0 += ko) {
-    const int64_t k = std::min(ko, nouter - o0);
-    for (int64_t c0 = 0; c0 < ninner; c0 += nb) {
-      const int64_t n = std::min(nb, ninner - c0);
-      char* in;
-      WB2_TRY(pipe.next(&in));
-      void* out[4] = {nullptr, nullptr, nullptr, nullptr};
-      char* op = in + b_in;
-      for (int s = 0; s < 4; ++s)
-        if (out_host[s]) {
-          out[s] = op;
-          op += b_out;
-        }
-      // the band's series: k * ntime rows of n cells, one strided 2-D copy
-      WB2_TRY(pipe.h2d_2d(in, size_t(n) * es, xh + (size_t(o0) * ntime * ninner + c0) * es,
-                          size_t(ninner) * es, size_t(n) * es, size_t(k) * ntime));
-      WB2_TRY(pipe.ready());
-      WB2_TRY(tw_launch_any(ctx, dtype, in, k, ntime, n, nbin, d_start, d_count, window, skipna,
-                            out));
-      for (int s = 0; s < 4; ++s)
-        if (out_host[s])
-          WB2_TRY(pipe.d2h_2d(out_host[s] + (size_t(o0) * nout * ninner + c0) * es,
-                              size_t(ninner) * es, out[s], size_t(n) * es, size_t(n) * es,
-                              size_t(k) * nout));
-      WB2_TRY(pipe.done());
-    }
-  }
-  return pipe.finish();
+  return stream_series_bands(
+      ctx, x, dtype == WB2_F32 ? 4 : 8, nouter, ntime, ninner, nout, out_host, 4, budget,
+      [&](const void* in, int64_t k, int64_t n, void* const* out) {
+        return tw_launch_any(ctx, dtype, in, k, ntime, n, nbin, d_start, d_count, window,
+                             skipna, out);
+      });
 }
 
 }  // extern "C"

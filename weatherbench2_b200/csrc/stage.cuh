@@ -3,6 +3,7 @@
 // small host tables into device blocks the entry owns.
 #pragma once
 
+#include <algorithm>
 #include <initializer_list>
 
 #include "common.cuh"
@@ -130,6 +131,60 @@ class DeviceBlock {
   char* p_ = nullptr;
   cudaStream_t stream_ = nullptr;
 };
+
+// Streams a HOST series [nouter][ntime][ninner] of `es`-byte values through a
+// private staging pair in bands: inner cells of one outer index, or whole
+// outer indices when one fits `budget` (the device bytes of both buffers, at
+// least one cell per band).  Each band is one strided 2-D copy of k outer x n
+// inner cells; `launch(in, k, n, dev_out)` runs its kernels on ctx->stream,
+// reading `in` as [k][ntime][n] and writing dev_out[s] as [k][nout][n] for
+// every s whose out_host[s] is not NULL; those are copied back into
+// out_host[s], host [nouter][nout][ninner].  nout_host <= 4.
+template <typename Launch>
+int stream_series_bands(wb2_ctx* ctx, const void* x, size_t es, int64_t nouter, int64_t ntime,
+                        int64_t ninner, int64_t nout, char* const* out_host, int nout_host,
+                        size_t budget, Launch&& launch) {
+  int nstat = 0;
+  for (int s = 0; s < nout_host; ++s) nstat += out_host[s] != nullptr;
+  const size_t per_cell = (size_t(ntime) + size_t(nstat) * nout) * es;
+  const int64_t cells = std::max<int64_t>(1, static_cast<int64_t>(budget / (2 * per_cell)));
+  const int64_t nb = std::min(cells, ninner);
+  const int64_t ko = nb == ninner ? std::max<int64_t>(1, std::min(cells / ninner, nouter)) : 1;
+  auto al = [](size_t b) { return (b + 255) / 256 * 256; };
+  const size_t b_in = al(size_t(ko) * nb * ntime * es), b_out = al(size_t(ko) * nb * nout * es);
+  const size_t stage_bytes = b_in + nstat * b_out;
+
+  StagePair stage;
+  WB2_TRY(stage.alloc(stage_bytes));
+  StagePipe pipe(ctx, stage.buf[0], stage.buf[1]);
+  const char* xh = static_cast<const char*>(x);
+  for (int64_t o0 = 0; o0 < nouter; o0 += ko) {
+    const int64_t k = std::min(ko, nouter - o0);
+    for (int64_t c0 = 0; c0 < ninner; c0 += nb) {
+      const int64_t n = std::min(nb, ninner - c0);
+      char* in;
+      WB2_TRY(pipe.next(&in));
+      void* out[4] = {nullptr, nullptr, nullptr, nullptr};
+      char* op = in + b_in;
+      for (int s = 0; s < nout_host; ++s)
+        if (out_host[s]) {
+          out[s] = op;
+          op += b_out;
+        }
+      WB2_TRY(pipe.h2d_2d(in, size_t(n) * es, xh + (size_t(o0) * ntime * ninner + c0) * es,
+                          size_t(ninner) * es, size_t(n) * es, size_t(k) * ntime));
+      WB2_TRY(pipe.ready());
+      WB2_TRY(launch(static_cast<const void*>(in), k, n, static_cast<void* const*>(out)));
+      for (int s = 0; s < nout_host; ++s)
+        if (out_host[s])
+          WB2_TRY(pipe.d2h_2d(out_host[s] + (size_t(o0) * nout * ninner + c0) * es,
+                              size_t(ninner) * es, out[s], size_t(n) * es, size_t(n) * es,
+                              size_t(k) * nout));
+      WB2_TRY(pipe.done());
+    }
+  }
+  return pipe.finish();
+}
 
 struct HostPart {
   const void* src;  // may be NULL when bytes == 0

@@ -4,9 +4,11 @@ spectrum and the circumference scaling run in csrc/spectrum.cu.
 The wind variables of derived_variables.py:59-338 -- wind speed, divergence,
 vorticity, vertical velocity and the geostrophic / ageostrophic winds -- live in
 _derived_wind.py (csrc/derived.cu, csrc/wind_dynamics.cu) and are re-exported
-here.  The remaining derived variables of the reference (eddy kinetic energy,
-lapse rate, column integrals, relative humidity, precipitation accumulations)
-are not reproduced.
+here.  The precipitation accumulations of derived_variables.py:471-528 and
+685-720 live in _derived_precip.py (csrc/precip_accumulation.cu,
+csrc/resample.cu) and are re-exported here.  The remaining derived variables
+of the reference (eddy kinetic energy, lapse rate, column integrals, relative
+humidity) are not reproduced.
 """
 from __future__ import annotations
 
@@ -298,14 +300,16 @@ from weatherbench2_b200._derived_wind import (  # noqa: E402  pylint: disable=wr
     VComponentOfGeostrophicWind, VerticalVelocity, WindDivergence,
     WindSpeed, WindVorticity, _3DWindVariable, _AgeostrophicWindVariable,
     _GeostrophicWindVariable)
+from weatherbench2_b200._derived_precip import (  # noqa: E402  pylint: disable=wrong-import-position
+    AggregatePrecipitationAccumulation, PrecipitationAccumulation)
 
 # The named derived variables of weatherbench2/derived_variables.py:724-773 that
-# have a device implementation: wind speed and the horizontal-derivative
-# family (divergence, vorticity, vertical velocity, geostrophic and
-# ageostrophic winds).  The remaining entries of the reference's table (eddy
-# kinetic energy, lapse rate, column integrals, relative humidity,
-# precipitation accumulations) are not reproduced; asking for one raises
-# KeyError here instead of silently running on the host.
+# have a device implementation: wind speed, the horizontal-derivative family
+# (divergence, vorticity, vertical velocity, geostrophic and ageostrophic
+# winds) and the precipitation accumulations.  The remaining entries of the
+# reference's table (eddy kinetic energy, lapse rate, column integrals,
+# relative humidity) are not reproduced; asking for one raises KeyError here
+# instead of silently running on the host.
 DERIVED_VARIABLE_DICT = {
     'wind_speed': WindSpeed(u_name='u_component_of_wind',
                             v_name='v_component_of_wind'),
@@ -320,4 +324,24 @@ DERIVED_VARIABLE_DICT = {
     'ageostrophic_wind_speed': AgeostrophicWindSpeed(),
     'u_component_of_ageostrophic_wind': UComponentOfAgeostrophicWind(),
     'v_component_of_ageostrophic_wind': VComponentOfAgeostrophicWind(),
+    'total_precipitation_6hr': PrecipitationAccumulation(
+        total_precipitation_name='total_precipitation',
+        accumulation_hours=6,
+        lead_time_name='prediction_timedelta',
+    ),
+    'total_precipitation_24hr': PrecipitationAccumulation(
+        total_precipitation_name='total_precipitation',
+        accumulation_hours=24,
+        lead_time_name='prediction_timedelta',
+    ),
+    'total_precipitation_24hr_from_6hr': AggregatePrecipitationAccumulation(
+        accumulation_hours=24,
+        lead_time_name='prediction_timedelta',
+    ),
+    'total_precipitation_24hr_from_12hr': AggregatePrecipitationAccumulation(
+        accumulation_hours=24,
+        lead_time_name='prediction_timedelta',
+        raw_accumulation_name='total_precipitation_12hr',
+        raw_accumulation_hours=12,
+    ),
 }

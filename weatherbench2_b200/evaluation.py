@@ -65,6 +65,12 @@ def select_truth_at_valid_time(truth: xl.Dataset, forecast: xl.Dataset
   LazyGather view whose label lookup is folded into the kernels' offset table.
   """
   vt = forecast['valid_time']
+  # like xarray's sel with a DataArray indexer, the result carries the
+  # indexer's coordinates (init_time and lead_time, which derived variables
+  # along lead time read)
+  extra = {k: c for k, c in forecast.coords.items()
+           if c.dims and all(d in vt.dims for d in c.dims)}
+  extra['valid_time'] = xl.Coord(vt.dims, vt.values)
   out = xl.Dataset(attrs=truth.attrs)
   for k in truth.keys():
     v = truth[k]
@@ -73,8 +79,7 @@ def select_truth_at_valid_time(truth: xl.Dataset, forecast: xl.Dataset
       continue
     pos = xl._lookup(v.coords['time'].values, vt.values.ravel())  # pylint: disable=protected-access
     out[k] = LazyGather(v, {'time': (vt.dims, pos.reshape(vt.shape))},
-                        extra_coords={'valid_time': xl.Coord(vt.dims,
-                                                             vt.values)})
+                        extra_coords=extra)
   return out
 
 
