@@ -14,6 +14,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel resample --steps 5
   python benchmarks/bench_kernels.py --kernel wind_dynamics --steps 20
   python benchmarks/bench_kernels.py --kernel precip_accumulation --steps 20
+  python benchmarks/bench_kernels.py --kernel quantile --steps 5
 """
 import argparse
 import json
@@ -687,13 +688,103 @@ def bench_precip_accumulation(args):
       torch_pageable_roundtrip_ms=rt * 1e3)), flush=True)
 
 
+def _torch_sort_quantile(torch, x, q):
+  """What a user would write without the kernel: torch.sort along the sample
+  dim, then a gather of the order statistics and numpy's lerp (no NaN)."""
+  n = x.shape[1]
+  v = [(n - 1) * float(k) for k in q]
+  i = [min(int(np.floor(t)), n - 1) for t in v]
+  j = [min(k + 1, n - 1) for k in i]
+  g = torch.tensor([t - k for t, k in zip(v, i)], device=x.device,
+                   dtype=torch.float64).view(1, -1, 1)
+  s = torch.sort(x, dim=1).values
+  a = s.index_select(1, torch.tensor(i, device=x.device)).double()
+  b = s.index_select(1, torch.tensor(j, device=x.device)).double()
+  return a + (b - a) * g
+
+
+def bench_quantile(args):
+  """wb2_quantile on device-resident float32 series against torch.sort plus a
+  gather in the same run: an ensemble (n = 50), one year of 6-hourly steps
+  (n = 1460, also with 1 and 20 quantiles), 30 years at 1.5 degrees
+  (n = 43,828), the longitude axis (ninner = 1); then a 13-level year streamed
+  from host NumPy.  Bytes: the input once plus the float64 output once."""
+  import time
+  torch, _lib, ctx = setup()
+  card = _card()
+  q5 = [0.01, 0.1, 0.5, 0.9, 0.99]
+  ncell = NLAT * NLON
+  cases = [('ensemble 4x50x721x1440', (4, 50, ncell), q5),
+           ('one year 1460x721x1440', (1, 1460, ncell), q5),
+           ('one year 1460x721x1440 nq=1', (1, 1460, ncell), [0.5]),
+           ('one year 1460x721x1440 nq=20', (1, 1460, ncell),
+            list(np.linspace(0.025, 0.975, 20))),
+           ('1990-2019 43828x121x240', (1, 43828, 121 * 240), q5),
+           ('longitude (1460x721)x1440x1', (1460 * 721, 1440, 1), q5)]
+  gen = torch.Generator(device='cuda').manual_seed(0)
+  for name, (nouter, n, ninner), q in cases:
+    x = torch.empty((nouter, n, ninner), device='cuda').normal_(
+        1e5, 1.0, generator=gen)
+    out = torch.empty((len(q), nouter, ninner), device='cuda',
+                      dtype=torch.float64)
+    fn = lambda: ctx.quantile(x.data_ptr(), _lib.F32, nouter, n, ninner,  # noqa: E731
+                              q, False, out.data_ptr())
+    nbytes = x.numel() * 4 + out.numel() * 8
+    ms = timeit(fn, args.steps)
+    report(f'quantile device {name} nq={len(q)}', ms, nbytes,
+           nouter * ninner, 'cells', dict(card, nsample=n))
+    if 'nq=' not in name:
+      ref = _torch_sort_quantile(torch, x, q)
+      got = out.permute(1, 0, 2)
+      assert torch.equal(torch.isnan(got), torch.isnan(ref)), name
+      del ref, got
+      torch.cuda.empty_cache()
+      try:
+        ms = timeit(lambda: _torch_sort_quantile(torch, x, q),  # noqa: E731
+                    max(1, args.steps // 2), warmup=1)
+        report(f'torch.sort + gather {name} nq={len(q)}', ms, nbytes,
+               nouter * ninner, 'cells', dict(card, nsample=n))
+      except torch.cuda.OutOfMemoryError:
+        print(json.dumps(dict(card, kernel=f'torch.sort + gather {name}',
+                              ms=None, error='out of memory')), flush=True)
+    del x, out
+    torch.cuda.empty_cache()
+  from weatherbench2_b200 import preprocessing
+  n, ninner = 1460, 13 * 121 * 240
+  xh = torch.empty((1, n, ninner), device='cuda').normal_(
+      280.0, 10.0, generator=gen).cpu().numpy()
+  oh = np.empty((len(q5), 1, ninner))
+  run = lambda: ctx.quantile_host(  # noqa: E731
+      xh.ctypes.data, _lib.F32, 1, n, ninner, q5, False,
+      preprocessing.QUANTILE_STREAM_BUDGET_BYTES, oh.ctypes.data)
+  run()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    run()
+  s = (time.perf_counter() - t0) / args.steps
+  dev = torch.empty(xh.size, device='cuda')
+  src = torch.from_numpy(xh.reshape(-1))
+  dev.copy_(src)
+  torch.cuda.synchronize()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    dev.copy_(src)
+  torch.cuda.synchronize()
+  h2d = (time.perf_counter() - t0) / args.steps
+  print(json.dumps(dict(
+      card, kernel='quantile streamed host 1460x13x121x240 nq=5',
+      ms=s * 1e3, algorithmic_GB=(xh.nbytes + oh.nbytes) / 1e9,
+      torch_pageable_h2d_ms=h2d * 1e3)), flush=True)
+
+
 if __name__ == '__main__':
   ap = argparse.ArgumentParser()
   ap.add_argument('--kernel', required=True,
                   choices=['ens', 'energy', 'det', 'regrid', 'spectrum',
                            'maps', 'threshold', 'climatology',
                            'climatology_quantile', 'resample',
-                           'wind_dynamics', 'precip_accumulation'])
+                           'wind_dynamics', 'precip_accumulation',
+                           'quantile'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -705,4 +796,5 @@ if __name__ == '__main__':
    'climatology_quantile': bench_climatology_quantile,
    'resample': bench_resample,
    'wind_dynamics': bench_wind_dynamics,
-   'precip_accumulation': bench_precip_accumulation}[a.kernel](a)
+   'precip_accumulation': bench_precip_accumulation,
+   'quantile': bench_quantile}[a.kernel](a)

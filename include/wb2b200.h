@@ -520,6 +520,42 @@ int wb2_precip_accumulation_host(wb2_ctx* ctx, const void* x, int dtype, int64_t
                                  int64_t ntime, int64_t ninner, int32_t window,
                                  int clamp_negative, size_t budget, void* out);
 
+/* ---- quantiles over a sample axis ---------------------------------------------------
+ * wb2_quantile replaces xarray's Dataset.quantile(q, dim, skipna) (method 'linear'),
+ * the computation of scripts/compute_quantiles.py:168-183.  x is
+ * [nouter][nsample][ninner] (float32 or float64, read in place); quantiles is a HOST
+ * array of nquantile float64 values in [0, 1]; out is device
+ * [nquantile][nouter][ninner] float64.  Per cell, with T the data type, the result is
+ * numpy's np.quantile (skipna 0) / np.nanquantile (skipna 1) with float64 q, bit for
+ * bit:
+ *   1. skipna 0 and any sample NaN: every output NaN.  skipna 1: NaN samples are
+ *      dropped.  m = the samples left; m = 0 gives NaN for every output.
+ *   2. s = the m samples sorted ascending (equal values in any order).
+ *   3. v = double(m - 1) * q, correctly rounded.  v >= m - 1: i = j = m - 1 and
+ *      g = v + 1 (numpy's previous index -1).  Otherwise i = floor(v), j = i + 1,
+ *      g = v - i.
+ *   4. d = T(s[j] - s[i]), rounded in T.
+ *   5. g < 0.5: out = double(s[i]) + double(d) * g; else
+ *      out = double(s[j]) - double(d) * (1 - g); each operation a separately rounded
+ *      double operation, none contracted.
+ *   6. out is float64 for both data types.
+ * So [inf] gives NaN, [1, inf] NaN at q = 0 and q = 1, and float32 [1, 16777218]
+ * gives 8388610 at q = 0.5.  Only the sign of a zero read from samples whose +-0
+ * order is undefined may differ from numpy.  Argument errors (each names the
+ * argument; nothing is launched): dtype, nsample < 1, nquantile outside 1..128, a
+ * quantile outside [0, 1] or NaN, a NULL pointer.  nsample and the ranks are 64-bit;
+ * nouter * ninner = 0 is a no-op.  One kernel launch per call.                      */
+int wb2_quantile(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter, int64_t nsample,
+                 int64_t ninner, int32_t nquantile, const double* quantiles, int skipna,
+                 double* out);
+
+/* wb2_quantile on a HOST series (NumPy / memmap), streamed in bands like
+ * wb2_time_window_stats_host within `budget` device bytes; out is a host array of
+ * the same [nquantile][nouter][ninner] layout.  One launch per band.               */
+int wb2_quantile_host(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter,
+                      int64_t nsample, int64_t ninner, int32_t nquantile,
+                      const double* quantiles, int skipna, size_t budget, double* out);
+
 /* ---- K10: rank histogram ---------------------------------------------------------
  * Replaces RankHistogram.compute_chunk (metrics.py:1894-2042) and the time mean
  * of EnsembleMetric.compute: rank of the truth among the members (NaN last),

@@ -201,7 +201,15 @@ PROTOTYPES = {
     'wb2_precip_accumulation_host': (C.c_int, [
         _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int,
         C.c_size_t, _P]),
+    'wb2_quantile': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
+        C.POINTER(C.c_double), C.c_int, _P]),
+    'wb2_quantile_host': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
+        C.POINTER(C.c_double), C.c_int, C.c_size_t, _P]),
 }
+# wb2_quantile: quantiles per call
+MAX_QUANTILES = 128
 # wb2_climatology_quantile: quantiles per call, nitem * window_size per window
 CLIM_MAX_QUANTILES = 16
 CLIM_QUANTILE_MAX_SAMPLES = 8192
@@ -767,6 +775,37 @@ class Context:
         self.handle, _P(x) if x else None, dtype, int(nouter), int(ntime),
         int(ninner), int(window), int(bool(clamp_negative)), int(budget),
         _P(out) if out else None))
+
+  # -- quantiles over a sample axis --------------------------------------------
+  @staticmethod
+  def _quantile_list(quantiles):
+    if quantiles is None:
+      return 0, None, None
+    q = np.ascontiguousarray(quantiles, dtype=np.float64).reshape(-1)
+    return int(q.size), _as_ptr(q, C.c_double), q
+
+  def quantile(self, x: int, dtype: int, nouter: int, nsample: int,
+               ninner: int, quantiles, skipna: bool, out: int,
+               nquantile: Optional[int] = None):
+    """x and out are DEVICE addresses (wb2_quantile); quantiles a host
+    sequence of float64 (`nquantile` overrides its length)."""
+    nq, qp, keep = self._quantile_list(quantiles)
+    check(self.lib.wb2_quantile(
+        self.handle, _P(x) if x else None, dtype, int(nouter), int(nsample),
+        int(ninner), nq if nquantile is None else int(nquantile), qp,
+        int(bool(skipna)), _P(out) if out else None))
+    del keep
+
+  def quantile_host(self, x: int, dtype: int, nouter: int, nsample: int,
+                    ninner: int, quantiles, skipna: bool, budget: int,
+                    out: int, nquantile: Optional[int] = None):
+    """x and out are HOST addresses (wb2_quantile_host)."""
+    nq, qp, keep = self._quantile_list(quantiles)
+    check(self.lib.wb2_quantile_host(
+        self.handle, _P(x) if x else None, dtype, int(nouter), int(nsample),
+        int(ninner), nq if nquantile is None else int(nquantile), qp,
+        int(bool(skipna)), int(budget), _P(out) if out else None))
+    del keep
 
   # -- K10 --------------------------------------------------------------------
   def rank_histogram(self, x: int, t: int, nmember: int, member_stride: int,

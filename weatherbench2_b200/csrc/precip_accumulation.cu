@@ -223,8 +223,9 @@ int wb2_precip_accumulation_host(wb2_ctx* ctx, const void* x, int dtype, int64_t
   WB2_REQUIRE(out != nullptr, "out is NULL");
   DeviceGuard guard(ctx->device);
   char* const out_host[1] = {static_cast<char*>(out)};
+  const size_t es = dtype == WB2_F32 ? 4 : 8;
   return stream_series_bands(
-      ctx, x, dtype == WB2_F32 ? 4 : 8, nouter, ntime, ninner, ntime, out_host, 1, budget,
+      ctx, x, es, es, nouter, ntime, ninner, ntime, false, out_host, 1, budget,
       [&](const void* in, int64_t k, int64_t n, void* const* dev_out) {
         return pa_launch_any(ctx, dtype, in, k, ntime, n, window, clamp_negative, dev_out[0]);
       });

@@ -387,8 +387,9 @@ int wb2_time_window_stats_host(wb2_ctx* ctx, const void* x, int dtype, int64_t n
   const int64_t* d_start;
   const int32_t* d_count;
   WB2_TRY(tw_upload(ctx, nbin, bin_start, bin_count, &tables, &d_start, &d_count));
+  const size_t es = dtype == WB2_F32 ? 4 : 8;
   return stream_series_bands(
-      ctx, x, dtype == WB2_F32 ? 4 : 8, nouter, ntime, ninner, nout, out_host, 4, budget,
+      ctx, x, es, es, nouter, ntime, ninner, nout, false, out_host, 4, budget,
       [&](const void* in, int64_t k, int64_t n, void* const* out) {
         return tw_launch_any(ctx, dtype, in, k, ntime, n, nbin, d_start, d_count, window,
                              skipna, out);

@@ -139,19 +139,24 @@ class DeviceBlock {
 // inner cells; `launch(in, k, n, dev_out)` runs its kernels on ctx->stream,
 // reading `in` as [k][ntime][n] and writing dev_out[s] as [k][nout][n] for
 // every s whose out_host[s] is not NULL; those are copied back into
-// out_host[s], host [nouter][nout][ninner].  nout_host <= 4.
+// out_host[s], host [nouter][nout][ninner].  nout_host <= 4.  Outputs are
+// `out_es`-byte values.  With `out_major` the band outputs are [nout][k][n]
+// instead and the host outputs [nout][nouter][ninner]: a band is part of one
+// outer index or whole outer indices, so its cells are one contiguous run of
+// every host plane and come back in one 2-D copy.
 template <typename Launch>
-int stream_series_bands(wb2_ctx* ctx, const void* x, size_t es, int64_t nouter, int64_t ntime,
-                        int64_t ninner, int64_t nout, char* const* out_host, int nout_host,
-                        size_t budget, Launch&& launch) {
+int stream_series_bands(wb2_ctx* ctx, const void* x, size_t es, size_t out_es, int64_t nouter,
+                        int64_t ntime, int64_t ninner, int64_t nout, bool out_major,
+                        char* const* out_host, int nout_host, size_t budget, Launch&& launch) {
   int nstat = 0;
   for (int s = 0; s < nout_host; ++s) nstat += out_host[s] != nullptr;
-  const size_t per_cell = (size_t(ntime) + size_t(nstat) * nout) * es;
+  const size_t per_cell = size_t(ntime) * es + size_t(nstat) * nout * out_es;
   const int64_t cells = std::max<int64_t>(1, static_cast<int64_t>(budget / (2 * per_cell)));
   const int64_t nb = std::min(cells, ninner);
   const int64_t ko = nb == ninner ? std::max<int64_t>(1, std::min(cells / ninner, nouter)) : 1;
   auto al = [](size_t b) { return (b + 255) / 256 * 256; };
-  const size_t b_in = al(size_t(ko) * nb * ntime * es), b_out = al(size_t(ko) * nb * nout * es);
+  const size_t b_in = al(size_t(ko) * nb * ntime * es);
+  const size_t b_out = al(size_t(ko) * nb * nout * out_es);
   const size_t stage_bytes = b_in + nstat * b_out;
 
   StagePair stage;
@@ -175,11 +180,17 @@ int stream_series_bands(wb2_ctx* ctx, const void* x, size_t es, int64_t nouter, 
                           size_t(ninner) * es, size_t(n) * es, size_t(k) * ntime));
       WB2_TRY(pipe.ready());
       WB2_TRY(launch(static_cast<const void*>(in), k, n, static_cast<void* const*>(out)));
-      for (int s = 0; s < nout_host; ++s)
-        if (out_host[s])
-          WB2_TRY(pipe.d2h_2d(out_host[s] + (size_t(o0) * nout * ninner + c0) * es,
-                              size_t(ninner) * es, out[s], size_t(n) * es, size_t(n) * es,
-                              size_t(k) * nout));
+      for (int s = 0; s < nout_host; ++s) {
+        if (!out_host[s]) continue;
+        if (out_major)
+          WB2_TRY(pipe.d2h_2d(out_host[s] + (size_t(o0) * ninner + c0) * out_es,
+                              size_t(nouter) * ninner * out_es, out[s],
+                              size_t(k) * n * out_es, size_t(k) * n * out_es, size_t(nout)));
+        else
+          WB2_TRY(pipe.d2h_2d(out_host[s] + (size_t(o0) * nout * ninner + c0) * out_es,
+                              size_t(ninner) * out_es, out[s], size_t(n) * out_es,
+                              size_t(n) * out_es, size_t(k) * nout));
+      }
       WB2_TRY(pipe.done());
     }
   }
