@@ -15,6 +15,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel wind_dynamics --steps 20
   python benchmarks/bench_kernels.py --kernel precip_accumulation --steps 20
   python benchmarks/bench_kernels.py --kernel quantile --steps 5
+  python benchmarks/bench_kernels.py --kernel average --steps 5
 """
 import argparse
 import json
@@ -777,6 +778,121 @@ def bench_quantile(args):
       torch_pageable_h2d_ms=h2d * 1e3)), flush=True)
 
 
+def bench_average(args):
+  """wb2_average against (x * w).nansum / count in torch, per statistic, in the
+  same run: a global latitude-weighted mean of 1464 steps at 721 x 1440 (K R),
+  (time, longitude) means of 124 steps x 13 levels (R K R), a time-mean map
+  (R K), all three raw moments over (longitude, latitude), one cell over the
+  whole array; then 1464 steps x 13 x 121 x 240 streamed from host NumPy, next
+  to the pageable host-to-device rate.  Bytes: the input once plus the
+  outputs once; the share is of the data sheet's 3.35 TB/s unless a measured
+  peak is given."""
+  import time
+  torch, _lib, ctx = setup()
+  from weatherbench2_b200 import _spatial as sp
+  card = _card()
+  gen = torch.Generator(device='cuda').manual_seed(0)
+  ncell = NLAT * NLON
+  w_lat = sp.lat_weights(np.linspace(-90, 90, NLAT))
+
+  def field(shape):
+    x = torch.empty(shape, device='cuda', dtype=torch.float32)
+    flat = x.view(-1)
+    for i in range(0, flat.numel(), 1 << 28):
+      flat[i:i + (1 << 28)].normal_(280.0, 10.0, generator=gen)
+    flat[::1000003] = float('nan')
+    return x
+
+  def run(name, x, shape, stats, base, weights=None, wdiv=1):
+    k0, _, k1, _, k2 = shape
+    dt = torch.float64 if weights is not None else torch.float32
+    outs = {s: torch.empty(k0 * k1 * k2, device='cuda',
+                           dtype=torch.float64 if s == 'frac' else dt)
+            for s in stats}
+    fn = lambda: ctx.average(x.data_ptr(), _lib.F32, shape, True,  # noqa: E731
+                             **{s: o.data_ptr() for s, o in outs.items()},
+                             weights=weights, wdiv=wdiv)
+    nbytes = x.numel() * 4 + sum(o.numel() * o.element_size()
+                                 for o in outs.values())
+    ms = timeit(fn, args.steps, warmup=1)
+    report(f'average device {name}', ms, nbytes, x.numel(), 'samples',
+           dict(card, shape=list(shape), stats=list(stats)))
+    ref = base()
+    for s, r in zip(stats, ref):
+      torch.testing.assert_close(outs[s].double(), r.reshape(-1).double(),
+                                 rtol=1e-5, atol=1e-6, equal_nan=True)
+    del ref
+    torch.cuda.empty_cache()
+    ms = timeit(base, max(1, args.steps // 2), warmup=1)
+    report(f'torch nansum / count {name}', ms, nbytes, x.numel(), 'samples',
+           card)
+
+  # global latitude-weighted mean per step: [1464][721 * 1440]
+  x = field((1464, NLAT, NLON))
+  wt = torch.from_numpy(w_lat).cuda()[:, None]
+
+  def base_global():
+    cnt = (~x.isnan()).sum((1, 2))
+    return [(x * wt).nansum((1, 2)) / cnt]
+  run('global lat-weighted mean 1464x721x1440 (K R)', x,
+      (1464, ncell, 1, 1, 1), ('mean',), base_global, w_lat, NLON)
+  del x
+  torch.cuda.empty_cache()
+  # [124 time][13 level][721][1440]
+  x = field((124, 13, NLAT, NLON))
+
+  def base_tlon():
+    return [x.nansum((0, 3)) / (~x.isnan()).sum((0, 3))]
+  run('(time, longitude) 124x13x721x1440 (R K R)', x,
+      (1, 124, 13 * NLAT, NLON, 1), ('mean',), base_tlon)
+
+  def base_tmap():
+    return [x.nansum(0) / (~x.isnan()).sum(0)]
+  run('time-mean map 124x13x721x1440 (R K)', x, (1, 124, 1, 1, 13 * ncell),
+      ('mean',), base_tmap)
+
+  def base_moments():
+    cnt = (~x.isnan()).sum((2, 3))
+    return [x.nansum((2, 3)) / cnt, (x * x).nansum((2, 3)) / cnt,
+            cnt.double() / ncell]
+  run('three moments 124x13x721x1440 (K R)', x, (124 * 13, ncell, 1, 1, 1),
+      ('mean', 'mean_sq', 'frac'), base_moments)
+
+  def base_all():
+    return [x.nansum() / (~x.isnan()).sum()]
+  run('reduce-all 124x13x721x1440 (one cell)', x, (1, x.numel(), 1, 1, 1),
+      ('mean',), base_all)
+  del x
+  torch.cuda.empty_cache()
+  # streamed from host NumPy: (time, longitude) of [1464][13][121][240]
+  from weatherbench2_b200 import preprocessing
+  shape = (1, 1464, 13 * 121, 240, 1)
+  xh = field((1464, 13, 121, 240)).cpu().numpy()
+  oh = np.empty(13 * 121, np.float32)
+  runh = lambda: ctx.average_host(  # noqa: E731
+      xh.ctypes.data, _lib.F32, shape, True,
+      preprocessing.AVERAGE_STREAM_BUDGET_BYTES, mean=oh.ctypes.data)
+  runh()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    runh()
+  s = (time.perf_counter() - t0) / args.steps
+  dev = torch.empty(xh.size, device='cuda')
+  src = torch.from_numpy(xh.reshape(-1))
+  dev.copy_(src)
+  torch.cuda.synchronize()
+  t0 = time.perf_counter()
+  for _ in range(args.steps):
+    dev.copy_(src)
+  torch.cuda.synchronize()
+  h2d = xh.nbytes / ((time.perf_counter() - t0) / args.steps) / 1e9
+  gbs = xh.nbytes / s / 1e9
+  print(json.dumps(dict(
+      card, kernel='average streamed host (time, longitude) 1464x13x121x240',
+      ms=s * 1e3, algorithmic_GB=xh.nbytes / 1e9, achieved_GBps=gbs,
+      h2d_pageable_GBps=h2d, frac_of_h2d=gbs / h2d)), flush=True)
+
+
 if __name__ == '__main__':
   ap = argparse.ArgumentParser()
   ap.add_argument('--kernel', required=True,
@@ -784,7 +900,7 @@ if __name__ == '__main__':
                            'maps', 'threshold', 'climatology',
                            'climatology_quantile', 'resample',
                            'wind_dynamics', 'precip_accumulation',
-                           'quantile'])
+                           'quantile', 'average'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -797,4 +913,5 @@ if __name__ == '__main__':
    'resample': bench_resample,
    'wind_dynamics': bench_wind_dynamics,
    'precip_accumulation': bench_precip_accumulation,
-   'quantile': bench_quantile}[a.kernel](a)
+   'quantile': bench_quantile,
+   'average': bench_average}[a.kernel](a)

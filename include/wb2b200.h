@@ -556,6 +556,52 @@ int wb2_quantile_host(wb2_ctx* ctx, const void* x, int dtype, int64_t nouter,
                       int64_t nsample, int64_t ninner, int32_t nquantile,
                       const double* quantiles, int skipna, size_t budget, double* out);
 
+/* ---- means and raw moments over reduced dims ----------------------------------------
+ * wb2_average replaces the `v * weights` + xbeam.Mean(dims, skipna) of
+ * scripts/compute_averages.py and the means of compute_statistical_moments.py's
+ * moment_reduce.  x (float32 or float64 T, read in place) is [k0][r0][k1][r1][k2]: the
+ * k extents are kept, the r extents reduced (any extent may be 1).  Per kept cell
+ * (k0, k1, k2), with n = r0 * r1 samples x[s] in the flat order s = r0' * r1 + r1':
+ *   w[s]     weights == NULL: 1; else the HOST float64 table weights[(s / wdiv) % wlen]
+ *            (wdiv * wlen must divide n)
+ *   y[s]     double(x[s]) * w[s], one float64 multiply
+ *   z[s]     double(T(x[s] * x[s])) * w[s]: the square is rounded in T as np.square
+ *            does (a float32 square may overflow to inf)
+ *   skipna 1 a NaN x[s] contributes +0.0 to both sums; skipna 0 it propagates
+ *   N        the number of non-NaN x[s]; count = N (skipna 1) or n (skipna 0)
+ *   mean     = S1 / count, mean_sq = S2 / count, frac = N / n (float64 divisions)
+ * The divisor is the count, not sum w: the reference's `v * weights` + xbeam.Mean.
+ * A cell with count 0 gives NaN; Inf follows IEEE float64 (inf + -inf is NaN).
+ * S1 (S2 likewise) is summed in float64 in this order, fixed by n alone:
+ *   1. the samples are cut into chunks of 65536 consecutive s;
+ *   2. in a chunk, class c (0..31) adds y[s] for s = chunk start + c, + 32, ... in
+ *      increasing s to an accumulator starting at +0.0;
+ *   3. the 32 class sums are added pairwise: a[c] + a[c + 16] for c < 16, then the
+ *      same with 8, 4, 2, 1 (a xor butterfly), giving the chunk's partial;
+ *   4. the partials are added in chunk order starting from +0.0.
+ * No addition chain is longer than ceil(n / 32) + 7, so the sum is within
+ * (ceil(n / 32) + 7) 2^-53 sum |y[s]| of the exact sum of the y[s] (to first order).
+ * Outputs (device arrays [k0][k1][k2]; each may be NULL, not all three): mean and
+ * mean_sq are float64 when weighted, else T, each rounded once from the float64
+ * quotient; frac is float64.  Argument errors (each names the argument; nothing is
+ * launched): dtype, r0 or r1 < 1, a negative kept extent, weights that do not fit
+ * the sample index, no output requested, a NULL pointer.  k0 * k1 * k2 = 0 is a
+ * no-op.  One kernel launch per call when n <= 65536, else three.                 */
+int wb2_average(wb2_ctx* ctx, const void* x, int dtype, int64_t k0, int64_t r0, int64_t k1,
+                int64_t r1, int64_t k2, const double* weights, int64_t wdiv, int64_t wlen,
+                int skipna, void* mean, void* mean_sq, double* frac);
+
+/* wb2_average on a HOST array (NumPy / memmap), streamed through two staging buffers
+ * within `budget` device bytes.  Bands hold whole cells: whole k0 slabs, else k1
+ * slices [r0][m][r1][k2] of one k0, else k2 cells [r0][r1][nb] of one (k0, k1); the
+ * outputs are host arrays of the same layout, bit-equal to wb2_average's.  Only a
+ * budget below one cell (its r0 * r1 samples, outputs and chunk partials, twice) is
+ * an error naming it.  The device entry's launches per band.                       */
+int wb2_average_host(wb2_ctx* ctx, const void* x, int dtype, int64_t k0, int64_t r0,
+                     int64_t k1, int64_t r1, int64_t k2, const double* weights, int64_t wdiv,
+                     int64_t wlen, int skipna, size_t budget, void* mean, void* mean_sq,
+                     double* frac);
+
 /* ---- K10: rank histogram ---------------------------------------------------------
  * Replaces RankHistogram.compute_chunk (metrics.py:1894-2042) and the time mean
  * of EnsembleMetric.compute: rank of the truth among the members (NaN last),

@@ -207,7 +207,17 @@ PROTOTYPES = {
     'wb2_quantile_host': (C.c_int, [
         _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
         C.POINTER(C.c_double), C.c_int, C.c_size_t, _P]),
+    'wb2_average': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+        C.c_int64, C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int, _P,
+        _P, _P]),
+    'wb2_average_host': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+        C.c_int64, C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int,
+        C.c_size_t, _P, _P, _P]),
 }
+# wb2_average: samples per chunk of the fixed summation order
+AVERAGE_CHUNK = 65536
 # wb2_quantile: quantiles per call
 MAX_QUANTILES = 128
 # wb2_climatology_quantile: quantiles per call, nitem * window_size per window
@@ -805,6 +815,42 @@ class Context:
         self.handle, _P(x) if x else None, dtype, int(nouter), int(nsample),
         int(ninner), nq if nquantile is None else int(nquantile), qp,
         int(bool(skipna)), int(budget), _P(out) if out else None))
+    del keep
+
+  # -- means and raw moments over reduced dims ---------------------------------
+  @staticmethod
+  def _average_args(shape, weights):
+    if len(shape) != 5:
+      raise ValueError(f'shape must be (k0, r0, k1, r1, k2) (got {shape})')
+    if weights is None:
+      return [int(s) for s in shape], None, None
+    w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+    return [int(s) for s in shape], _as_ptr(w, C.c_double), w
+
+  def average(self, x: int, dtype: int, shape, skipna: bool, mean: int = 0,
+              mean_sq: int = 0, frac: int = 0, weights=None, wdiv: int = 1,
+              wlen: Optional[int] = None):
+    """x and the outputs are DEVICE addresses (wb2_average); `shape` is the
+    canonical (k0, r0, k1, r1, k2); `weights` a host float64 table indexed by
+    (s / wdiv) % wlen (`wlen` defaults to its length); 0 skips an output."""
+    sh, wp, keep = self._average_args(shape, weights)
+    wl = (0 if keep is None else keep.size) if wlen is None else int(wlen)
+    check(self.lib.wb2_average(
+        self.handle, _P(x) if x else None, dtype, *sh, wp, int(wdiv), wl,
+        int(bool(skipna)), _P(mean) if mean else None,
+        _P(mean_sq) if mean_sq else None, _P(frac) if frac else None))
+    del keep
+
+  def average_host(self, x: int, dtype: int, shape, skipna: bool, budget: int,
+                   mean: int = 0, mean_sq: int = 0, frac: int = 0,
+                   weights=None, wdiv: int = 1, wlen: Optional[int] = None):
+    """x and the outputs are HOST addresses (wb2_average_host)."""
+    sh, wp, keep = self._average_args(shape, weights)
+    wl = (0 if keep is None else keep.size) if wlen is None else int(wlen)
+    check(self.lib.wb2_average_host(
+        self.handle, _P(x) if x else None, dtype, *sh, wp, int(wdiv), wl,
+        int(bool(skipna)), int(budget), _P(mean) if mean else None,
+        _P(mean_sq) if mean_sq else None, _P(frac) if frac else None))
     del keep
 
   # -- K10 --------------------------------------------------------------------

@@ -56,6 +56,19 @@ class StagePipe {
     ctx_->stat_h2d_bytes += int64_t(width * rows);
     return WB2_OK;
   }
+  // `slices` planes of `rows` rows of `width` bytes into dst, packed; in the
+  // source, rows are `spitch` bytes apart and planes `spitch * srows`.
+  int h2d_3d(void* dst, const void* src, size_t spitch, size_t srows, size_t width, size_t rows,
+             size_t slices) {
+    cudaMemcpy3DParms p = {};
+    p.srcPtr = make_cudaPitchedPtr(const_cast<void*>(src), spitch, width, srows);
+    p.dstPtr = make_cudaPitchedPtr(dst, width, width, rows);
+    p.extent = make_cudaExtent(width, rows, slices);
+    p.kind = cudaMemcpyHostToDevice;
+    WB2_CUDA_TRY(cudaMemcpy3DAsync(&p, ctx_->copy_stream));
+    ctx_->stat_h2d_bytes += int64_t(width * rows * slices);
+    return WB2_OK;
+  }
   int ready() {
     WB2_CUDA_TRY(cudaEventRecord(ctx_->stage_copied[cur_], ctx_->copy_stream));
     WB2_CUDA_TRY(cudaStreamWaitEvent(ctx_->stream, ctx_->stage_copied[cur_], 0));

@@ -1,9 +1,11 @@
 """Device-side preprocessing that feeds the metric kernels (SURVEY.md section 8
 f3): the ensemble mean of scripts/compute_ensemble_mean.py:110-141
 (`xbeam.Mean(realization, skipna)`) computed in HBM, so that ensemble-mean
-RMSE / ACC through K1 need no host round trip of the mean; and the quantiles
+RMSE / ACC through K1 need no host round trip of the mean; the quantiles
 of scripts/compute_quantiles.py (`Dataset.quantile` over chosen dims,
-csrc/quantile.cu)."""
+csrc/quantile.cu); and the area-weighted averages and raw moments of
+scripts/compute_averages.py and compute_statistical_moments.py
+(csrc/average.cu)."""
 from __future__ import annotations
 
 import math
@@ -187,7 +189,19 @@ def compute_quantiles(ds, quantiles: Sequence[float], dim, *,
   `levels` on `level`, each only where the dim exists), then
   `compute_quantiles_core`."""
   native = xl.is_native_xarray(ds)
-  ds = xl.from_xarray(ds)
+  ds = _impose_data_selection(xl.from_xarray(ds), variables, levels, time_dim,
+                              time_start, time_stop)
+  out = compute_quantiles_core(ds, quantiles, dim, skipna=skipna,
+                               name_suffix=name_suffix)
+  return xl.to_xarray(out) if native else out
+
+
+def _impose_data_selection(ds: xl.Dataset, variables, levels, time_dim,
+                           time_start, time_stop) -> xl.Dataset:
+  """`_impose_data_selection` of scripts/compute_quantiles.py and
+  compute_averages.py: `variables`, then [time_start, time_stop] on
+  `time_dim` with both ends inclusive, then `levels` on `level`, each only
+  where the dim exists."""
   if variables is not None:
     ds = ds[list(variables)]
   if time_dim in ds.dims:
@@ -195,6 +209,219 @@ def compute_quantiles(ds, quantiles: Sequence[float], dim, *,
     ds = ds.isel({time_dim: index.slice_indexer(time_start, time_stop)})
   if levels and 'level' in ds.dims:
     ds = ds.sel(level=[float(l) for l in levels])
-  out = compute_quantiles_core(ds, quantiles, dim, skipna=skipna,
-                               name_suffix=name_suffix)
+  return ds
+
+
+# -- means and raw moments over reduced dims (csrc/average.cu) -----------------
+MOMENT = 'moment'
+MOMENT_ORDERS = ('zeroth', 'first', 'second')
+# device bytes of the two staging buffers of a host (NumPy) average call
+AVERAGE_STREAM_BUDGET_BYTES = 1 << 30
+_STATS = ('mean', 'mean_sq', 'frac')
+
+
+def _average_layout(v: xl.DataArray, reduce: list):
+  """The canonical (k0, r0, k1, r1, k2) of `v` reduced over `reduce`, the
+  permutation that makes it one (None: `v` is read in place) and the reduced
+  dims in sample order.  Adjacent dims of the same kind are merged; a reduced
+  set of three or more runs is moved in front by one transposed copy."""
+  runs = []  # [is_reduced, [dims]]
+  for d in v.dims:
+    r = d in reduce
+    if runs and runs[-1][0] == r:
+      runs[-1][1].append(d)
+    else:
+      runs.append([r, [d]])
+  perm = None
+  if sum(r for r, _ in runs) > 2:
+    red = [d for d in v.dims if d in reduce]
+    keep = [d for d in v.dims if d not in reduce]
+    perm = [v.dims.index(d) for d in red + keep]
+    runs = [[True, red]] + ([[False, keep]] if keep else [])
+  # K R K or K R K R K; the last kept run is always k2, which the kernels
+  # read coalesced across cells
+  if runs[0][0]:
+    runs.insert(0, [False, []])
+  if runs[-1][0]:
+    runs.append([False, []])
+  if len(runs) == 3:
+    runs[2:2] = [[False, []], [True, []]]
+  shape = tuple(math.prod(v.sizes[d] for d in dims) for _, dims in runs)
+  sample_dims = runs[1][1] + runs[3][1]
+  return shape, perm, sample_dims
+
+
+def _check_average(v: xl.DataArray, reduce):
+  if not reduce:
+    raise ValueError(f'variable {v.name!r}: the dims to average over are '
+                     f'empty ({list(reduce)})')
+  if v.dtype not in (np.float32, np.float64):
+    raise TypeError(f'variable {v.name!r} has dtype {v.dtype}: averages '
+                    'take float32 or float64 data')
+  for d in reduce:
+    if d not in v.dims:
+      raise ValueError(f'variable {v.name!r} has no dimension {d!r} to '
+                       f'average over (dims {v.dims})')
+  if any(v.sizes[d] == 0 for d in reduce):
+    raise ValueError(f'variable {v.name!r}: cannot average over an empty '
+                     f'reduction ({reduce})')
+
+
+def _variable_average(v: xl.DataArray, reduce: list, stats, *, skipna: bool,
+                      weights=None, weight_dim: str = 'latitude'):
+  """{stat: array} of `v` over the dims `reduce` for each stat of `stats`
+  ('mean', 'mean_sq', 'frac'), shaped like the kept dims in input order: CUDA
+  tensors for CUDA data, else NumPy (streamed through the device in bands).
+  `weights` (a float64 vector along `weight_dim`, which must be reduced)
+  multiplies every sample first; the divisor stays the sample count."""
+  _check_average(v, reduce)
+  shape, perm, sample_dims = _average_layout(v, reduce)
+  wkw = {}
+  if weights is not None:
+    i = sample_dims.index(weight_dim)
+    wkw = dict(weights=np.asarray(weights, np.float64),
+               wdiv=math.prod(v.sizes[d] for d in sample_dims[i + 1:]))
+  keep_shape = tuple(v.sizes[d] for d in v.dims if d not in reduce)
+  dt = np.float64 if weights is not None else v.dtype
+  dtypes = {'mean': dt, 'mean_sq': dt, 'frac': np.float64}
+  code = _lib.F64 if v.dtype == np.float64 else _lib.F32
+  ctx = _lib.default_context()
+  data = v.data
+  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
+    import torch  # pylint: disable=import-outside-toplevel
+    x = (data if perm is None else data.permute(*perm)).contiguous()
+    out = {s: torch.empty(keep_shape, device=x.device,
+                          dtype=getattr(torch, np.dtype(dtypes[s]).name))
+           for s in stats}
+    if x.numel():
+      ctx.average(x.data_ptr(), code, shape, skipna,
+                  **{s: t.data_ptr() for s, t in out.items()}, **wkw)
+    return out
+  x = np.asarray(data)
+  x = np.ascontiguousarray(x if perm is None else np.transpose(x, perm))
+  out = {s: ctx.pinned_result(keep_shape, dtypes[s]) for s in stats}
+  if x.size:
+    ctx.average_host(x.ctypes.data, code, shape, skipna,
+                     AVERAGE_STREAM_BUDGET_BYTES,
+                     **{s: a.ctypes.data for s, a in out.items()}, **wkw)
+  return out
+
+
+def _kept_coords(ds: xl.Dataset, dims) -> dict:
+  return {k: c for k, c in ds.coords.items()
+          if not any(d in dims for d in c.dims)}
+
+
+def compute_averages(ds, averaging_dims: Sequence[str], *,
+                     skipna: bool = False,
+                     variables: Optional[Sequence[str]] = None,
+                     levels: Optional[Sequence] = None,
+                     time_dim: str = 'time',
+                     time_start: Optional[str] = '2020-01-01',
+                     time_stop: Optional[str] = '2020-12-31'):
+  """scripts/compute_averages.py `main` without Beam or zarr: the script's
+  `_impose_data_selection`, then per variable `v * weights` (when `latitude`
+  is averaged: metrics.get_lat_weights of the selected dataset) followed by
+  xbeam.Mean(averaging_dims, skipna).
+
+  Like that Mean, the divisor is the number of samples counted (all of them,
+  or the non-NaN ones with skipna), not the sum of the weights; with
+  get_lat_weights (mean 1) and no NaN the two agree.  The result is float64
+  when weighted (the reference's float32 * float64 product), else the data
+  type; it keeps the other dims in input order, drops coordinates along
+  averaged dims and has no attrs.  A variable without one of the averaging
+  dims raises ValueError.  CUDA-tensor variables give CUDA tensors; NumPy or
+  memmap variables are streamed through the device and give NumPy.  Sums are
+  float64 in the order include/wb2b200.h fixes (DESIGN.md section 8g)."""
+  native = xl.is_native_xarray(ds)
+  ds = _impose_data_selection(xl.from_xarray(ds), variables, levels, time_dim,
+                              time_start, time_stop)
+  dims = [averaging_dims] if isinstance(averaging_dims, str) else list(
+      averaging_dims)
+  weights = None
+  if 'latitude' in dims:
+    from weatherbench2_b200 import metrics  # pylint: disable=import-outside-toplevel
+    weights = metrics.get_lat_weights(ds).values
+  for name in ds.keys():
+    _check_average(ds[name], dims)
+  out = xl.Dataset(coords=_kept_coords(ds, dims))
+  for name in ds.keys():
+    v = ds[name]
+    res = _variable_average(v, dims, ('mean',), skipna=skipna,
+                            weights=weights)
+    out[name] = xl.DataArray(res['mean'],
+                             tuple(d for d in v.dims if d not in dims))
+  return xl.to_xarray(out) if native else out
+
+
+def _moment_stat(order: str) -> str:
+  try:
+    return _STATS[('first', 'second', 'zeroth').index(order)]
+  except ValueError:
+    raise NotImplementedError(f'Order {order} not implemented.') from None
+
+
+def moment_reduce(obs, order: str = 'first',
+                  reduce_dims: Sequence[str] = ('longitude', 'latitude'),
+                  sel_kwargs: Optional[dict] = None):
+  """`moment_reduce` of scripts/compute_statistical_moments.py: the mean over
+  `reduce_dims` of the data (order 'first'), of its square rounded in the
+  data type (np.square, 'second') or of its non-NaN mask ('zeroth': the
+  fraction of non-NaN samples, float64).  Unweighted and NaN-skipping, as
+  xarray's mean of float data is; other orders raise NotImplementedError."""
+  stat = _moment_stat(order)
+  native = xl.is_native_xarray(obs)
+  ds = xl.from_xarray(obs)
+  if sel_kwargs:
+    ds = ds.sel(sel_kwargs)
+  dims = [reduce_dims] if isinstance(reduce_dims, str) else list(reduce_dims)
+  for name in ds.keys():
+    _check_average(ds[name], dims)
+  out = xl.Dataset(coords=_kept_coords(ds, dims))
+  for name in ds.keys():
+    v = ds[name]
+    res = _variable_average(v, dims, (stat,), skipna=True)
+    out[name] = xl.DataArray(res[stat],
+                             tuple(d for d in v.dims if d not in dims))
+  return xl.to_xarray(out) if native else out
+
+
+def compute_statistical_moments(obs, *, start_year: Optional[int] = 1990,
+                                end_year: Optional[int] = 2020,
+                                time_dim: str = 'time'):
+  """scripts/compute_statistical_moments.py `main` without Beam or zarr: the
+  years start_year..end_year (both inclusive) of `time_dim`, then per
+  variable the zeroth, first and second raw moments over longitude and
+  latitude (one read of the data for all three), then their mean over time.
+
+  The spatial moments are kept in the dtypes the reference materialises (the
+  data type, the data type, float64) before the time mean, which skips NaN
+  steps.  The result has variables `{var}_{order}`, order-major as the
+  script's template, with dims ('moment', *rest): `moment` has size 1 and no
+  coordinate."""
+  native = xl.is_native_xarray(obs)
+  ds = xl.from_xarray(obs)
+  if start_year is not None and end_year is not None:
+    index = pd.Index(ds.coords[time_dim].values)
+    ds = ds.isel({time_dim: index.slice_indexer(str(start_year),
+                                                str(end_year))})
+  space = ['longitude', 'latitude']
+  gone = space + [time_dim]
+  out = xl.Dataset(coords=_kept_coords(ds, gone))
+  for name in ds.keys():
+    _check_average(ds[name], gone)
+  results = {}
+  for name in ds.keys():
+    v = ds[name]
+    spatial = _variable_average(v, space, _STATS, skipna=True)
+    sdims = tuple(d for d in v.dims if d not in space)
+    rest = tuple(d for d in sdims if d != time_dim)
+    for order in MOMENT_ORDERS:
+      s = xl.DataArray(spatial[_moment_stat(order)], sdims, name=name)
+      m = _variable_average(s, [time_dim], ('mean',), skipna=True)['mean']
+      results[(order, name)] = (m.reshape((1,) + tuple(m.shape)), rest)
+  for order in MOMENT_ORDERS:
+    for name in ds.keys():
+      values, rest = results[(order, name)]
+      out[f'{name}_{order}'] = xl.DataArray(values, (MOMENT,) + rest)
   return xl.to_xarray(out) if native else out
