@@ -583,9 +583,10 @@ def _quiet():
 
 
 @contextlib.contextmanager
-def installed():
-  """Makes `_lib.default_context()` return a FakeContext inside the block."""
-  fake = FakeContext()
+def installed(cls=FakeContext):
+  """Makes `_lib.default_context()` return a `cls` (a FakeContext) inside the
+  block."""
+  fake = cls()
   saved = _lib.default_context
   _lib.default_context = lambda device=None: fake
   try:

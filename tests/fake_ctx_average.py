@@ -5,7 +5,6 @@ run end to end on a CPU.  It applies the entries' argument checks and
 tests/average_oracle.py to the canonical [k0][r0][k1][r1][k2] array the
 operators hand to the library (the kernels themselves are checked by the GPU
 tests)."""
-import contextlib
 import math
 
 import numpy as np
@@ -67,13 +66,6 @@ class AverageFakeContext(fake_ctx.FakeContext):
         _view(ptr, math.prod(a.shape), a.dtype)[...] = a.reshape(-1)
 
 
-@contextlib.contextmanager
 def installed():
   """Makes `_lib.default_context()` return an AverageFakeContext."""
-  fake = AverageFakeContext()
-  saved = _lib.default_context
-  _lib.default_context = lambda device=None: fake
-  try:
-    yield fake
-  finally:
-    _lib.default_context = saved
+  return fake_ctx.installed(AverageFakeContext)

@@ -4,8 +4,6 @@ that weatherbench2_b200.utils runs end to end on a CPU.  It reads the same
 index tables the operators hand to the library and applies the header's
 definitions tap by tap (the kernel's sliding sums and float64 shift are checked
 by the GPU tests)."""
-import contextlib
-
 import numpy as np
 
 import fake_ctx
@@ -79,13 +77,6 @@ class ClimatologyFakeContext(fake_ctx.FakeContext):
             np.float32).reshape(-1)
 
 
-@contextlib.contextmanager
 def installed():
   """Makes `_lib.default_context()` return a ClimatologyFakeContext."""
-  fake = ClimatologyFakeContext()
-  saved = _lib.default_context
-  _lib.default_context = lambda device=None: fake
-  try:
-    yield fake
-  finally:
-    _lib.default_context = saved
+  return fake_ctx.installed(ClimatologyFakeContext)

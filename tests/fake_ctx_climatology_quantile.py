@@ -5,10 +5,9 @@ operators of weatherbench2_b200.utils run end to end on a CPU.  It reads the
 index tables the operators hand to the library and applies the header's
 definitions to every window at once, cells vectorised (the kernel's sliding
 sorted window is checked by the GPU tests)."""
-import contextlib
-
 import numpy as np
 
+import fake_ctx
 import fake_ctx_climatology
 from fake_ctx import _quiet, _view
 from weatherbench2_b200 import _lib
@@ -98,13 +97,6 @@ class QuantileFakeContext(fake_ctx_climatology.ClimatologyFakeContext):
           np.float32).ravel()
 
 
-@contextlib.contextmanager
 def installed():
   """Makes `_lib.default_context()` return a QuantileFakeContext."""
-  fake = QuantileFakeContext()
-  saved = _lib.default_context
-  _lib.default_context = lambda device=None: fake
-  try:
-    yield fake
-  finally:
-    _lib.default_context = saved
+  return fake_ctx.installed(QuantileFakeContext)

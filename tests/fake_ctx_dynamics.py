@@ -5,8 +5,6 @@ strides and the gradient-coefficient / cos / Coriolis / pressure tables the
 operators hand to the library and applies the header's arithmetic to them in
 float64 NumPy (which never fuses a multiply-add), so the CPU tests check both
 the tables and the arithmetic contract against tests/dynamics_oracle.py."""
-import contextlib
-
 import numpy as np
 
 import fake_ctx
@@ -106,13 +104,6 @@ class DynamicsFakeContext(fake_ctx.FakeContext):
     _view(out, n, np.float32)[...] = r.reshape(-1)
 
 
-@contextlib.contextmanager
 def installed():
   """Makes `_lib.default_context()` return a DynamicsFakeContext."""
-  fake = DynamicsFakeContext()
-  saved = _lib.default_context
-  _lib.default_context = lambda device=None: fake
-  try:
-    yield fake
-  finally:
-    _lib.default_context = saved
+  return fake_ctx.installed(DynamicsFakeContext)

@@ -5,10 +5,9 @@ derived variables run end to end on a CPU.  It applies the entry's argument
 checks and tests/precip_oracle.py to the [outer][time][inner] series the
 operators hand to the library (the kernel's staging and in-place differences
 are checked by the GPU tests)."""
-import contextlib
-
 import numpy as np
 
+import fake_ctx
 import fake_ctx_resample
 import precip_oracle as po
 from fake_ctx import _view
@@ -52,13 +51,6 @@ class PrecipFakeContext(fake_ctx_resample.ResampleFakeContext):
     _view(out, n, dt)[...] = res.reshape(-1)
 
 
-@contextlib.contextmanager
 def installed():
   """Makes `_lib.default_context()` return a PrecipFakeContext."""
-  fake = PrecipFakeContext()
-  saved = _lib.default_context
-  _lib.default_context = lambda device=None: fake
-  try:
-    yield fake
-  finally:
-    _lib.default_context = saved
+  return fake_ctx.installed(PrecipFakeContext)

@@ -4,8 +4,6 @@ preprocessing.compute_quantiles runs end to end on a CPU.  It applies the
 entries' argument checks and tests/quantile_oracle.py to the
 [outer][n][inner] series the operator hands to the library (the kernels'
 staging, sorting networks and radix select are checked by the GPU tests)."""
-import contextlib
-
 import numpy as np
 
 import fake_ctx
@@ -58,13 +56,6 @@ class QuantileFakeContext(fake_ctx.FakeContext):
     _view(out, nq * nouter * ninner, np.float64)[...] = res.reshape(-1)
 
 
-@contextlib.contextmanager
 def installed():
   """Makes `_lib.default_context()` return a QuantileFakeContext."""
-  fake = QuantileFakeContext()
-  saved = _lib.default_context
-  _lib.default_context = lambda device=None: fake
-  try:
-    yield fake
-  finally:
-    _lib.default_context = saved
+  return fake_ctx.installed(QuantileFakeContext)

@@ -5,8 +5,6 @@ on a CPU.  It reads the [outer][time][inner] series and the bin tables the
 operators hand to the library and applies the float64 oracle bin by bin (the
 kernels' staging, sliding sums and van Herk extrema are checked by the GPU
 tests)."""
-import contextlib
-
 import numpy as np
 
 import fake_ctx
@@ -50,13 +48,6 @@ class ResampleFakeContext(fake_ctx.FakeContext):
         _view(p, res[s].size, dt)[...] = res[s].astype(dt).reshape(-1)
 
 
-@contextlib.contextmanager
 def installed():
   """Makes `_lib.default_context()` return a ResampleFakeContext."""
-  fake = ResampleFakeContext()
-  saved = _lib.default_context
-  _lib.default_context = lambda device=None: fake
-  try:
-    yield fake
-  finally:
-    _lib.default_context = saved
+  return fake_ctx.installed(ResampleFakeContext)

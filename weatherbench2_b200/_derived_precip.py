@@ -17,7 +17,7 @@ import dataclasses
 
 import numpy as np
 
-from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import derived_variables as dv
 from weatherbench2_b200 import resampling
 from weatherbench2_b200 import xarray_lite as xl
@@ -50,25 +50,9 @@ def precip_accumulation(da: xl.DataArray, lead: str, window: int,
   nouter = int(np.prod(shape[:li], dtype=np.int64))
   ntime = shape[li]
   ninner = int(np.prod(shape[li + 1:], dtype=np.int64))
-  code = _lib.F64 if da.dtype == np.float64 else _lib.F32
-  ctx = _lib.default_context()
-  data = da.data
-  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    x = data.contiguous()
-    out = torch.empty(shape, dtype=x.dtype, device=x.device)
-    if out.numel():
-      ctx.precip_accumulation(x.data_ptr(), code, nouter, ntime, ninner,
-                              window, clamp_negative, out.data_ptr())
-    return out
-  x = np.ascontiguousarray(da.values)
-  out = ctx.pinned_result(shape, x.dtype)
-  if out.size:
-    ctx.precip_accumulation_host(x.ctypes.data, code, nouter, ntime, ninner,
-                                 window, clamp_negative,
-                                 resampling.STREAM_BUDGET_BYTES,
-                                 out.ctypes.data)
-  return out
+  return _streamed.run('precip_accumulation', da.data,
+                       (nouter, ntime, ninner, window, clamp_negative),
+                       [(shape, da.dtype)], resampling.STREAM_BUDGET_BYTES)[0]
 
 
 @dataclasses.dataclass

@@ -15,6 +15,7 @@ import numpy as np
 import pandas as pd
 
 from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import xarray_lite as xl
 
 REALIZATION = 'realization'
@@ -110,26 +111,11 @@ def _variable_quantiles(v: xl.DataArray, reduce: list, quantiles: list,
   else:
     nouter, ninner = 1, math.prod(v.sizes[d] for d in keep)
     perm = pos + [v.dims.index(d) for d in keep]
-  code = _lib.F64 if v.dtype == np.float64 else _lib.F32
-  nq = len(quantiles)
-  out_shape = (nq,) + tuple(v.sizes[d] for d in keep)
-  ctx = _lib.default_context()
-  data = v.data
-  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    x = (data if perm is None else data.permute(*perm)).contiguous()
-    out = torch.empty(out_shape, dtype=torch.float64, device=x.device)
-    if out.numel():
-      ctx.quantile(x.data_ptr(), code, nouter, nsample, ninner, quantiles,
-                   skipna, out.data_ptr())
-    return out
-  x = np.asarray(data)
-  x = np.ascontiguousarray(x if perm is None else np.transpose(x, perm))
-  out = ctx.pinned_result(out_shape, np.float64)
-  if out.size:
-    ctx.quantile_host(x.ctypes.data, code, nouter, nsample, ninner, quantiles,
-                      skipna, QUANTILE_STREAM_BUDGET_BYTES, out.ctypes.data)
-  return out
+  out_shape = (len(quantiles),) + tuple(v.sizes[d] for d in keep)
+  return _streamed.run('quantile', v.data,
+                       (nouter, nsample, ninner, quantiles, skipna),
+                       [(out_shape, np.float64)], QUANTILE_STREAM_BUDGET_BYTES,
+                       perm=perm)[0]
 
 
 def compute_quantiles_core(chunk, quantiles: Sequence[float], dim, *,
@@ -284,27 +270,12 @@ def _variable_average(v: xl.DataArray, reduce: list, stats, *, skipna: bool,
   keep_shape = tuple(v.sizes[d] for d in v.dims if d not in reduce)
   dt = np.float64 if weights is not None else v.dtype
   dtypes = {'mean': dt, 'mean_sq': dt, 'frac': np.float64}
-  code = _lib.F64 if v.dtype == np.float64 else _lib.F32
-  ctx = _lib.default_context()
-  data = v.data
-  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    x = (data if perm is None else data.permute(*perm)).contiguous()
-    out = {s: torch.empty(keep_shape, device=x.device,
-                          dtype=getattr(torch, np.dtype(dtypes[s]).name))
-           for s in stats}
-    if x.numel():
-      ctx.average(x.data_ptr(), code, shape, skipna,
-                  **{s: t.data_ptr() for s, t in out.items()}, **wkw)
-    return out
-  x = np.asarray(data)
-  x = np.ascontiguousarray(x if perm is None else np.transpose(x, perm))
-  out = {s: ctx.pinned_result(keep_shape, dtypes[s]) for s in stats}
-  if x.size:
-    ctx.average_host(x.ctypes.data, code, shape, skipna,
-                     AVERAGE_STREAM_BUDGET_BYTES,
-                     **{s: a.ctypes.data for s, a in out.items()}, **wkw)
-  return out
+  res = _streamed.run(
+      'average', v.data, (shape, skipna),
+      [(keep_shape, dtypes[s]) if s in stats else None for s in _STATS],
+      AVERAGE_STREAM_BUDGET_BYTES, perm=perm, **wkw)
+  res = dict(zip(_STATS, res))
+  return {s: res[s] for s in stats}
 
 
 def _kept_coords(ds: xl.Dataset, dims) -> dict:

@@ -32,7 +32,7 @@ from typing import Optional, Sequence
 import numpy as np
 import pandas as pd
 
-from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import xarray_lite as xl
 
 STATISTICS = ('mean', 'min', 'max', 'sum')
@@ -94,27 +94,13 @@ def _stats(da: xl.DataArray, time_dim: str, stats: Sequence[str],
   start, count = bins if bins is not None else (None, None)
   nout = ntime if window else len(count)
   oshape = shape[:ti] + (nout,) + shape[ti + 1:]
-  code = _lib.F64 if da.dtype == np.float64 else _lib.F32
-  ctx = _lib.default_context()
-  data = da.data
-  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    x = data.contiguous()
-    res = {s: torch.empty(oshape, dtype=x.dtype, device=x.device)
-           for s in stats}
-    ptr = {s: res[s].data_ptr() if s in res else None for s in STATISTICS}
-    if nouter * ninner * nout:
-      ctx.time_window_stats(x.data_ptr(), code, nouter, ntime, ninner, start,
-                            count, window, skipna, *ptr.values())
-    return res
-  x = np.ascontiguousarray(da.values)
-  res = {s: ctx.pinned_result(oshape, x.dtype) for s in stats}
-  ptr = {s: res[s].ctypes.data if s in res else None for s in STATISTICS}
-  if nouter * ninner * nout:
-    ctx.time_window_stats_host(x.ctypes.data, code, nouter, ntime, ninner,
-                               start, count, window, skipna,
-                               STREAM_BUDGET_BYTES, *ptr.values())
-  return res
+  res = _streamed.run(
+      'time_window_stats', da.data,
+      (nouter, ntime, ninner, start, count, window, skipna),
+      [(oshape, da.dtype) if s in stats else None for s in STATISTICS],
+      STREAM_BUDGET_BYTES)
+  res = dict(zip(STATISTICS, res))
+  return {s: res[s] for s in stats}
 
 
 def _plan(times, method: str, period: pd.Timedelta, label_side: str):

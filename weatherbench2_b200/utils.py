@@ -45,6 +45,7 @@ import numpy as np
 import pandas as pd
 
 from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import xarray_lite as xl
 
 EXPLICIT, FAST = 0, 1
@@ -236,53 +237,34 @@ def _plan(times, clim_years, hours: Optional[Sequence[int]], method: int,
 
 # -- execution ------------------------------------------------------------------
 def _series(da: xl.DataArray, plan):
-  """(x, dtype code, other dims, their shape, ncell, ntime, on device): the
-  (time, cells) series the kernels read, float64 kept unless resampled."""
+  """(perm, dtype, other dims, their shape, ncell, ntime) of the (time, cells)
+  series the kernels read: time first, float64 kept unless resampled, every
+  other dtype read as float32."""
   ti = da.dims.index('time')
   other = tuple(d for d in da.dims if d != 'time')
   oshape = tuple(da.sizes[d] for d in other)
   ncell = int(np.prod(oshape)) if oshape else 1
-  ntime = da.sizes['time']
-  data = da.data
-  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    x = data.movedim(ti, 0)
-    if x.dtype != torch.float64 or plan.nres:
-      x = x.to(torch.float32)
-    x = x.contiguous()
-    code = _lib.F64 if x.dtype == torch.float64 else _lib.F32
-    return x, code, other, oshape, ncell, ntime, True
-  x = np.asarray(data)
-  if ti:
-    x = np.moveaxis(x, ti, 0)
-  dt = np.float64 if x.dtype == np.float64 and not plan.nres else np.float32
-  x = np.ascontiguousarray(x, dtype=dt)
-  code = _lib.F64 if dt == np.float64 else _lib.F32
-  return x, code, other, oshape, ncell, ntime, False
+  perm = [ti] + [i for i in range(len(da.dims)) if i != ti]
+  # by name: a CUDA tensor may hold a dtype NumPy lacks (bfloat16)
+  f64 = str(da.data.dtype).replace('torch.', '') == 'float64'
+  dt = np.float64 if f64 and not plan.nres else np.float32
+  return perm, dt, other, oshape, ncell, da.sizes['time']
 
 
 def _run(ds: xl.Dataset, plan, labels, hours, stats: Sequence[str]) -> dict:
   """{stat: {variable: DataArray}} for every variable with a time axis."""
-  ctx = _lib.default_context()
   out = {s: {} for s in stats}
   for name, da in ds.items():
     if 'time' not in da.dims:
       continue
-    x, code, other, oshape, ncell, ntime, device = _series(da, plan)
+    perm, dt, other, oshape, ncell, ntime = _series(da, plan)
     nrow = (plan.nhour, plan.nday_out)
-    if device:
-      import torch  # pylint: disable=import-outside-toplevel
-      res = {s: torch.empty(nrow + oshape, device=x.device,
-                            dtype=torch.float32) for s in stats}
-      ptr = {s: res[s].data_ptr() if s in res else None for s in ('mean', 'std')}
-      ctx.climatology(x.data_ptr(), code, ntime, ncell, plan, ptr['mean'],
-                      ptr['std'])
-    else:
-      res = {s: ctx.pinned_result(nrow + oshape, np.float32) for s in stats}
-      ptr = {s: res[s].ctypes.data if s in res else None
-             for s in ('mean', 'std')}
-      ctx.climatology_host(x.ctypes.data, code, ntime, ncell, plan,
-                           STREAM_BUDGET_BYTES, ptr['mean'], ptr['std'])
+    res = _streamed.run(
+        'climatology', da.data, (ntime, ncell, plan),
+        [(nrow + oshape, np.float32) if s in stats else None
+         for s in ('mean', 'std')], STREAM_BUDGET_BYTES, perm=perm, dtype=dt)
+    res = dict(zip(('mean', 'std'), res))
+    res = {s: res[s] for s in stats}
     coords = {k: c for k, c in da.coords.items() if 'time' not in c.dims}
     coords['dayofyear'] = xl.Coord(('dayofyear',), labels)
     if hours is None:
@@ -321,7 +303,6 @@ def _compute(obs, window_size: int, clim_years: slice,
 def _run_quantile(ds: xl.Dataset, plan, labels, hours, spec) -> dict:
   """{name: DataArray}: the quantiles of every variable with a time axis
   (names kept), or the SEEPS pair of `spec.var`."""
-  ctx = _lib.default_context()
   seeps = isinstance(spec, SEEPSThreshold)
   qs = np.array([2 / 3]) if seeps else _quantile_values(spec.quantiles)
   thr = spec.dry_threshold_m if seeps else None
@@ -331,23 +312,13 @@ def _run_quantile(ds: xl.Dataset, plan, labels, hours, spec) -> dict:
   out = {}
   for name in names:
     da = ds[name]
-    x, code, other, oshape, ncell, ntime, device = _series(da, plan)
+    perm, dt, other, oshape, ncell, ntime = _series(da, plan)
     qshape = (plan.nhour, qs.size, plan.nday_out) + oshape
     dshape = (plan.nhour, plan.nday_out) + oshape
-    if device:
-      import torch  # pylint: disable=import-outside-toplevel
-      res = torch.empty(qshape, device=x.device, dtype=torch.float32)
-      dry = (torch.empty(dshape, device=x.device, dtype=torch.float32)
-             if seeps else None)
-      ctx.climatology_quantile(x.data_ptr(), code, ntime, ncell, plan, qs, thr,
-                               res.data_ptr(),
-                               dry.data_ptr() if seeps else None)
-    else:
-      res = ctx.pinned_result(qshape, np.float32)
-      dry = ctx.pinned_result(dshape, np.float32) if seeps else None
-      ctx.climatology_quantile_host(x.ctypes.data, code, ntime, ncell, plan, qs,
-                                    thr, STREAM_BUDGET_BYTES, res.ctypes.data,
-                                    dry.ctypes.data if seeps else None)
+    res, dry = _streamed.run(
+        'climatology_quantile', da.data, (ntime, ncell, plan, qs, thr),
+        [(qshape, np.float32), (dshape, np.float32) if seeps else None],
+        STREAM_BUDGET_BYTES, perm=perm, dtype=dt)
     coords = {k: c for k, c in da.coords.items() if 'time' not in c.dims}
     coords['dayofyear'] = xl.Coord(('dayofyear',), labels)
     if hours is not None:
