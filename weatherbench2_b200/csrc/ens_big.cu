@@ -94,21 +94,28 @@ __global__ void __launch_bounds__(kBigThreads) ens_big_kernel(const BigParams p)
     sumx = warp_sum(sumx); suma = warp_sum(suma);
     nval = warp_sum(nval); naval = warp_sum(naval);
     const float mean = skipna ? sumx / nval : sumx / fm;
+    // ranks come from the raw tile values; each term is formed on the member
+    // relative to the mean, as in K2 (ens_point.cuh): a finite mean only
+    const bool finite_mean = fabsf(mean) <= __int_as_float(0x7f7fffff);
+    const float shift = finite_mean ? mean : 0.f;
     float ss = 0.f, s = 0.f;
     for (int m = lane; m < M; m += 32) {
       const float xm = tile[m * kBigPitch + c];
-      const float dx = xm - mean;
+      const float dx = xm - shift;
       if (!skipna || dx == dx) ss += dx * dx;
       // ordinal rank by counting (metrics.py:836-846)
       int rank = 1;
       for (int j = 0; j < M; ++j) rank += big_less(tile[j * kBigPitch + c], j, xm, m) ? 1 : 0;
-      const float term = (2.f * float(rank) - fm - 1.f) * xm;  // metrics.py:808
+      const float term = (2.f * float(rank) - fm - 1.f) * dx;  // metrics.py:808
       if (!skipna || xm == xm) s += term;
     }
     ss = warp_sum(ss);
     s = warp_sum(s);
+    // the n valid ranks' coefficients add up to n (n - M) (skipna, see ens_point)
+    if (skipna) s += shift * (nval * (nval - fm));
     float val[kBigStats];
-    const float var = skipna ? (nval > 1.f ? ss / (nval - 1.f) : nanv) : ss / (fm - 1.f);
+    const float var = !finite_mean ? nanv
+                      : skipna ? (nval > 1.f ? ss / (nval - 1.f) : nanv) : ss / (fm - 1.f);
     const float dm = t - mean;
     val[0] = skipna ? suma / naval : suma / fm;
     val[1] = M < 2 ? 0.f : (skipna ? 2.f * (s / nval) / (fm - 1.f) : 2.f * (s / fm) / (fm - 1.f));

@@ -112,8 +112,8 @@ constexpr bool kTwinSortOk = EXACT && !SKIPNA && MP >= 8 && MP % 2 == 0;
 //   [0] skill_pt  = mean_m |t - x_m|                          (metrics.py:824)
 //   [1] spread_pt = 2 * mean_m((2 r_m - M - 1) x_m) / (M - 1) (metrics.py:805-813)
 //   [2] (t - xbar)^2          [3] var_m(x, ddof=1)     [4] [2] - [3] / M
-// TWIN: sort the mean-removed members with the packed network (the spread sum
-// is invariant to a common shift because its coefficients add up to zero).
+// Every path sorts the mean-removed members; TWIN sorts them with the packed
+// network, whose (a + b) - lo comparators round relative to the dispersion.
 template <int MP, bool SKIPNA, bool EXACT, bool TWIN = false>
 __device__ __forceinline__ void ens_point(float (&v)[MP], float t, int M, float (&val)[kEnsStats]) {
   static_assert(!TWIN || kTwinSortOk<MP, SKIPNA, EXACT>, "packed sort needs a full even ensemble");
@@ -142,23 +142,35 @@ __device__ __forceinline__ void ens_point(float (&v)[MP], float t, int M, float 
   // (ens_pair_kernel gained 9 % from the same change); <= 1 ulp apart.
   const float inv_m = EXACT ? 1.f / float(MP) : 1.f / fm;
   const float inv_m1 = EXACT ? 1.f / float(MP > 1 ? MP - 1 : 1) : 1.f / (fm - 1.f);
-  const float mean = SKIPNA ? sumx / nvalid : sumx * inv_m;  // 0/0 -> NaN like nanmean
+  // __fmul_rn: the mean is rounded once and subtracted from every member; a
+  // contracted x_m - sumx * inv_m would leave the residual of the rounded
+  // reciprocal, so that equal members had a variance > 0.
+  const float mean = SKIPNA ? sumx / nvalid : __fmul_rn(sumx, inv_m);  // 0/0 -> NaN like nanmean
+  // The members are kept relative to the mean: the rank sum below is formed
+  // on them, so its rounding scales with the ensemble's dispersion, not with
+  // |x| (5e4 +- 5 would lose about three digits of the spread otherwise).  An
+  // infinite or NaN mean (an infinite or, without skipna, NaN member) keeps
+  // the raw members, whose rank sum is the reference's +-inf / NaN; the
+  // variance is then NaN, like x - mean in the reference.
+  const bool finite_mean = fabsf(mean) <= __int_as_float(0x7f7fffff);
+  const float shift = finite_mean ? mean : 0.f;
   float ss = 0.f;
 #pragma unroll
   for (int m = 0; m < MP; ++m) {
     if (EXACT || m < M) {
-      const float dx = v[m] - mean;
+      const float dx = v[m] - shift;
       if (SKIPNA) {
         if (dx == dx) ss += dx * dx;
       } else {
         ss += dx * dx;
       }
-      if (TWIN) v[m] = dx;
+      v[m] = dx;
     }
   }
   float var;
-  if (SKIPNA) var = nvalid > 1.f ? ss / (nvalid - 1.f) : nanf_;  // np.nanvar(ddof=1)
-  else var = M > 1 ? ss * inv_m1 : ss / (fm - 1.f);              // M == 1 -> 0/0 = NaN
+  if (!finite_mean) var = nanf_;
+  else if (SKIPNA) var = nvalid > 1.f ? ss / (nvalid - 1.f) : nanf_;  // np.nanvar(ddof=1)
+  else var = M > 1 ? ss * inv_m1 : ss / (fm - 1.f);                 // M == 1 -> 0/0 = NaN
   const float dm = t - mean;
   const float mse = dm * dm;
   val[0] = SKIPNA ? suma / navalid : suma * inv_m;
@@ -189,6 +201,10 @@ __device__ __forceinline__ void ens_point(float (&v)[MP], float t, int M, float 
       s += coef * v[i];
     }
   }
+  // The coefficients of the n valid ranks add up to n (n - M): 0 for a full
+  // ensemble; under skipna with missing members the reference keeps M in
+  // them, and the shift's share comes back here.
+  if (SKIPNA) s += shift * (nvalid * (nvalid - fm));
   float spread = SKIPNA ? 2.f * (s / nvalid) * inv_m1 : 2.f * (s * inv_m) * inv_m1;
   if (!SKIPNA && !(sumx == sumx)) spread = nanf_;  // a NaN member poisons the point
   val[1] = spread;
