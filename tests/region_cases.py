@@ -350,7 +350,7 @@ def _det_plan(case, env, offsets_aligned=None):
   if case.nseg == 1:
     nstage = min(32, (220 * 1024 // (noper * stage_op)) // 4 * 4)
     return Plan('tma', 2) if nstage >= 8 else ldg
-  cw = 16 if env.get('WB2_SEG_WARPS') == '16' else 8
+  cw = 8
   rch = 8 if case.skipna else 16
   ns = (6 if case.clim else 3) + ((4 if case.clim else 1) if case.skipna else 1)
   bands = seg_bands(case.row_w, rch)
@@ -747,7 +747,7 @@ def exact_cases():
   rs = np.random.RandomState(20261015)
   cs = []
   tma_env = _det_env(True)
-  seg_env = ({}, {'WB2_SEG_WARPS': '16'}, {'WB2_DET_PATH': 'ldg'})
+  seg_env = ({}, {'WB2_DET_PATH': 'ldg'})
   # ---- K1 TMA, one segment -------------------------------------------------------
   for nrow, ncol, nfield in ((1, 128, 5), (2, 132, 3), (3, 1440, 2), (181, 128, 2)):
     for clim in (False, True):
@@ -777,7 +777,7 @@ def exact_cases():
           f'k1_seg_r{nreg}_sk{int(skipna)}', rs, nrow=24, ncol=128, nfield=3,
           nregion=nreg, seg_start=ss, skipna=skipna, nan_frac=0.04 * skipna,
           row_w=_banded_row_w(rs, 24, nreg, 5), env=seg_env,
-          covers=('k1_seg_chunks', 'seg_warps_16')))
+          covers=('k1_seg_chunks',)))
   cs.append(_det_case('k1_seg_128_bands', rs, nrow=128, ncol=128, nfield=2,
                       nregion=4, seg_start=[0, 64, 128],
                       row_w=_banded_row_w(rs, 128, 4, 128, 2), env=seg_env,
@@ -862,9 +862,7 @@ def exact_cases():
   cs.append(_ens_case('k2_skipna', rs, M=16, nrow=5, ncol=48, nregion=3,
                       skipna=True, nan_truth=0.1, covers=('k2_skipna',)))
   cs.append(_ens_case('k2_occ', rs, M=10, nrow=6, ncol=64, nregion=2,
-                      seg_start=[0, 30, 64],
-                      env=({'WB2_ENS_OCC': '4'}, {'WB2_ENS_OCC': '5'},
-                           {'WB2_ENS_OCC': '6'}), covers=('k2_occ',)))
+                      seg_start=[0, 30, 64]))
   cs.append(_ens_case('k2_weighted', rs, M=8, nrow=5, ncol=36, nregion=4,
                       seg_start=[0, 5, 6, 36], col_w=True, cell_w=True,
                       covers=('k2_weighted',)))
@@ -955,7 +953,6 @@ COVERAGE = {
     'k1_seg_zero_pattern': lambda c, p, ps: (
         p.path == 'tma_seg' and
         ((c.row_w == 0) & (np.abs(c.row_w).max(axis=0) > 0)[None]).any()),
-    'seg_warps_16': _any(lambda c, q: q.path == 'tma_seg' and q.cw == 16),
     'k1_ldg_residues': lambda c, p, ps: p.path == 'ldg' and p.vec == 4,
     'k1_ldg_short_segments': lambda c, p, ps: (
         p.path == 'ldg' and p.vec == 4 and
@@ -981,7 +978,6 @@ COVERAGE = {
                                  c.nmember in (8, 16, 32, 64)),
     'k2_inexact_mp': lambda c, p, ps: p.path == 'scalar' and c.nmember in (6, 33),
     'k2_skipna': lambda c, p, ps: p.path == 'scalar' and c.skipna,
-    'k2_occ': lambda c, p, ps: len(ps) == 3,
     'k2_weighted': lambda c, p, ps: (c.kind == 'ens' and c.nseg > 1 and
                                      c.col_w is not None and c.cell_w is not None),
     'k2_pair_odd_ncol': lambda c, p, ps: p.path == 'twin' and c.ncol % 2,

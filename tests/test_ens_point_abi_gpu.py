@@ -153,7 +153,7 @@ VARIANTS = {
 
 
 def _setenv(monkeypatch, env):
-  for k in ('WB2_ENS_PATH', 'WB2_ENS_SORT', 'WB2_ENS_OCC'):
+  for k in ('WB2_ENS_PATH', 'WB2_ENS_SORT'):
     monkeypatch.delenv(k, raising=False)
   for k, v in env.items():
     monkeypatch.setenv(k, v)
@@ -203,18 +203,6 @@ def test_ens_maps_points(ctx, M, skipna):
 
 def _bits(a):
   return np.ascontiguousarray(a).view(np.uint64 if a.dtype == np.float64 else np.uint32)
-
-
-@pytest.mark.parametrize('skipna', [False, True])
-@pytest.mark.parametrize('M', [10, 20, 51])
-def test_occupancy_variants_give_identical_bits(ctx, monkeypatch, M, skipna):
-  case = _case(M)
-  outs = []
-  for occ in ('4', '5', '6'):
-    _setenv(monkeypatch, {'WB2_ENS_PATH': 'scalar', 'WB2_ENS_OCC': occ})
-    outs.append(run_metrics(ctx, case, skipna))
-  np.testing.assert_array_equal(_bits(outs[0]), _bits(outs[1]))
-  np.testing.assert_array_equal(_bits(outs[0]), _bits(outs[2]))
 
 
 @pytest.mark.parametrize('M,variant', [(50, 'default'), (50, 'scalar'),

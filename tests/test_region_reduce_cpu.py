@@ -77,7 +77,6 @@ def test_dispatch_model(name):
 
 def test_dispatch_model_forced_paths():
   seg = EXACT['k1_seg_r17_sk0']
-  assert rc.plan(seg, {'WB2_SEG_WARPS': '16'}).cw == 16
   assert rc.plan(seg, {'WB2_DET_PATH': 'ldg'}).path == 'ldg'
   pair = EXACT['k2_pair_m16']
   assert rc.plan(pair, {'WB2_ENS_PATH': 'scalar'}).path == 'twin'

@@ -169,26 +169,3 @@ def test_pfa_full_size_parseval(monkeypatch):
   nyq = (xd[..., 0::2].sum(-1) - xd[..., 1::2].sum(-1)) / 1440
   np.testing.assert_allclose(got.sum(-1), (xd ** 2).mean(-1) + nyq ** 2, rtol=1e-5)
   _check(got[:1], _want(x[:1], scale))
-
-
-@pytest.mark.parametrize('plan', ['0', '1', '2', '4', 'd', 'w'])
-def test_alternative_cta_shapes_give_the_same_spectra(monkeypatch, plan):
-  """WB2_PFA_PLAN selects the CTA shape of the 1440-longitude kernel: '0' =
-  2 CTAs x 8 warps, '2' = 5 CTAs x 3 warps, 'w' = the warp-specialised pipeline
-  (one CTA per SM, stages as warp groups handing buffers over through
-  mbarriers -- measured slower than the default, kept as a documented
-  experiment, DESIGN.md).  All run the same arithmetic: identical results."""
-  from weatherbench2_b200 import _lib
-  ctx = _lib.default_context()
-  monkeypatch.setenv('WB2_SPECTRUM_PATH', 'pfa')
-  x, scale = _case(6, 45, 1440, seed=9)
-  base = _run(ctx, x, scale)
-  base_sum = _run(ctx, x, scale, accumulate=True, nslot=2)
-  base_red = _run_latsum(ctx, x, scale / 45, 3)
-  monkeypatch.setenv('WB2_PFA_PLAN', plan)
-  np.testing.assert_array_equal(_run(ctx, x, scale), base)
-  np.testing.assert_array_equal(_run(ctx, x, scale, accumulate=True, nslot=2),
-                                base_sum)
-  # the latitude reduction sums row groups of a different size per plan
-  np.testing.assert_allclose(_run_latsum(ctx, x, scale / 45, 3), base_red,
-                             rtol=2e-6)

@@ -360,12 +360,13 @@ int det_metrics_tma(wb2_ctx* ctx, bool clim, const void* f, const void* t, const
 // factor, nregion <= RCH (16; 8 with skipna) -- the host splits longer region
 // lists into several launches.
 
-// Consumer warps per CTA (template parameter CW below): 2 warps share a tile
-// (half a row each), so CW / 2 tiles are consumed at once.  The kernel is
-// partly latency-bound (dependent LDS -> FMA chains): 16 warps measured 3-7 %
-// faster than 8 in one run, but that shape has seen far less testing, so 8
-// stays the default and WB2_SEG_WARPS=16 is an opt-in tuning knob.
-constexpr int kSegDefaultWarps = 8;
+// Consumer warps per CTA (CW in the kernel): 2 warps share a tile (half a row
+// each), so CW / 2 tiles are consumed at once.  The kernel is partly
+// latency-bound (dependent LDS -> FMA chains): 16 warps measured 3-7 % faster
+// than 8 in one run, but that shape has seen far less testing, so it stays 8.
+constexpr int kSegWarps = 8;
+// regions per launch (RCH in the kernel); longer region lists take several
+constexpr int seg_regions(bool skipna) { return skipna ? 8 : 16; }
 constexpr int kSegDump = 16;  // tiles between band accumulator -> float64 dumps
 constexpr int kSegMaxBands = 128;  // row bands (runs of equal region patterns)
 constexpr int kSegMaxSpans = 64;  // spans per half row (two rounds of 32 lanes)
@@ -396,8 +397,10 @@ struct TmaSegParams {
   int32_t maxslots;
 };
 
-template <bool CLIM, bool SKIPNA, int RCH, int CW>
-__global__ void __launch_bounds__(((CW + 1) * 32), 1) det_tma_seg_kernel(const TmaSegParams p) {
+template <bool CLIM, bool SKIPNA>
+__global__ void __launch_bounds__(((kSegWarps + 1) * 32), 1)
+    det_tma_seg_kernel(const TmaSegParams p) {
+  constexpr int CW = kSegWarps, RCH = seg_regions(SKIPNA);
   constexpr int NOPER = CLIM ? 3 : 2;
   constexpr int NSUM = CLIM ? 6 : 3;
   // per-piece values: sums, then counts (skipna) or one cell count (!skipna)
@@ -572,14 +575,14 @@ __global__ void __launch_bounds__(((CW + 1) * 32), 1) det_tma_seg_kernel(const T
 // Returns 1 if the kernel ran, 0 if not eligible, < 0 on error.  Handles the
 // regions [r0, r0 + nreg) of `w`; `out` is the full [nfield][w->nregion][10]
 // array (this launch fills only its regions).
-template <int RCH, int CW>
 static int launch_seg(wb2_ctx* ctx, bool clim, bool skipna, const TmaSegParams& p, int ncta,
                       size_t smem) {
-  auto go = [&](auto kernel) { return launch_kernel(ctx, kernel, ncta, (CW + 1) * 32, smem, p); };
-  if (clim) return skipna ? go(det_tma_seg_kernel<true, true, RCH, CW>)
-                          : go(det_tma_seg_kernel<true, false, RCH, CW>);
-  return skipna ? go(det_tma_seg_kernel<false, true, RCH, CW>)
-                : go(det_tma_seg_kernel<false, false, RCH, CW>);
+  auto go = [&](auto kernel) {
+    return launch_kernel(ctx, kernel, ncta, (kSegWarps + 1) * 32, smem, p);
+  };
+  if (clim) return skipna ? go(det_tma_seg_kernel<true, true>)
+                          : go(det_tma_seg_kernel<true, false>);
+  return skipna ? go(det_tma_seg_kernel<false, true>) : go(det_tma_seg_kernel<false, false>);
 }
 
 __global__ void seg_scatter_kernel(const double* __restrict__ tmp, double* __restrict__ out,
@@ -595,9 +598,8 @@ int det_metrics_tma_seg(wb2_ctx* ctx, bool clim, const void* f, const void* t, c
                         const int64_t* d_off_c, const wb2_weights* w, int skipna, double* out) {
   const int noper = clim ? 3 : 2;
   if (w->ncol * 4 < 512 || w->ncol % 4 != 0) return 0;
-  const char* cw_env = getenv("WB2_SEG_WARPS");
-  const int CW = (cw_env && atoi(cw_env) == 16) ? 16 : kSegDefaultWarps;
-  const int rch = skipna ? 8 : 16;
+  constexpr int CW = kSegWarps;
+  const int rch = seg_regions(skipna);
   const int nsum = clim ? 6 : 3;
   const int ns = nsum + (skipna ? (clim ? 4 : 1) : 1);
   const int stage_op_bytes = (w->ncol * 4 + 127) / 128 * 128;
@@ -742,11 +744,7 @@ int det_metrics_tma_seg(wb2_ctx* ctx, bool clim, const void* f, const void* t, c
     p.nregion = nreg; p.nseg = w->nseg; p.zero_skip = w->zero_skip;
     p.nstage = nstage; p.stage_op_bytes = stage_op_bytes; p.maxslots = maxslots;
     WB2_CUDA_TRY(cudaMemsetAsync(p.partial, 0, part_bytes, ctx->stream));
-    int rc;
-    if (CW == 16) rc = skipna ? launch_seg<8, 16>(ctx, clim, true, p, ncta, smem)
-                              : launch_seg<16, 16>(ctx, clim, false, p, ncta, smem);
-    else rc = skipna ? launch_seg<8, 8>(ctx, clim, true, p, ncta, smem)
-                     : launch_seg<16, 8>(ctx, clim, false, p, ncta, smem);
+    const int rc = launch_seg(ctx, clim, skipna, p, ncta, smem);
     if (rc != WB2_OK) return rc;
     double* tmp = reinterpret_cast<double*>(reinterpret_cast<char*>(ctx->tma_partial) + part_bytes);
     const bool direct = (nreg == w->nregion);

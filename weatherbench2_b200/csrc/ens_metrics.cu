@@ -48,8 +48,10 @@ struct EnsParams {
   int32_t nblk;
 };
 
-template <int MP, bool SKIPNA, bool EXACT, int OCC, bool TWIN = false>
-__global__ void __launch_bounds__(kEnsThreads, OCC) ens_metrics_kernel(const EnsParams p) {
+// resident CTAs per SM the register allocation targets: 4 with skipna, 5 without
+template <int MP, bool SKIPNA, bool EXACT, bool TWIN = false>
+__global__ void __launch_bounds__(kEnsThreads, SKIPNA ? 4 : 5)
+    ens_metrics_kernel(const EnsParams p) {
   constexpr int NCNT = SKIPNA ? kEnsStats : 1;
   constexpr int NS = kEnsStats + NCNT;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -307,35 +309,17 @@ static int launch_ens(wb2_ctx* ctx, const EnsParams& p, int64_t nfield, bool ski
                       (p.col_w ? size_t(p.ncol) * sizeof(float) : 0);
   const dim3 grid(static_cast<unsigned>(nfield * p.nblk));
   auto go = [&](auto kernel) { return launch_kernel(ctx, kernel, grid, kEnsThreads, smem, p); };
-  // resident CTAs per SM the register allocation targets (tuning knob)
-  const char* occ_env = getenv("WB2_ENS_OCC");
-  const int occ = occ_env ? atoi(occ_env) : (skipna ? 4 : 5);
   // full even ensembles without NaN handling sort with the twin ((a + b) - lo)
   // network; WB2_ENS_SORT=exact keeps the pure min / max network
   if constexpr (kTwinSortOk<MP, false, true>) {
     const char* sort_env = getenv("WB2_ENS_SORT");
-    if (exact && !skipna && !(sort_env && strcmp(sort_env, "exact") == 0)) {
-      if (occ >= 6) return go(ens_metrics_kernel<MP, false, true, 6, true>);
-      if (occ == 5) return go(ens_metrics_kernel<MP, false, true, 5, true>);
-      return go(ens_metrics_kernel<MP, false, true, 4, true>);
-    }
+    if (exact && !skipna && !(sort_env && strcmp(sort_env, "exact") == 0))
+      return go(ens_metrics_kernel<MP, false, true, true>);
   }
-  if (occ >= 6) {
-    if (skipna) return exact ? go(ens_metrics_kernel<MP, true, true, 6>)
-                             : go(ens_metrics_kernel<MP, true, false, 6>);
-    return exact ? go(ens_metrics_kernel<MP, false, true, 6>)
-                 : go(ens_metrics_kernel<MP, false, false, 6>);
-  }
-  if (occ == 5) {
-    if (skipna) return exact ? go(ens_metrics_kernel<MP, true, true, 5>)
-                             : go(ens_metrics_kernel<MP, true, false, 5>);
-    return exact ? go(ens_metrics_kernel<MP, false, true, 5>)
-                 : go(ens_metrics_kernel<MP, false, false, 5>);
-  }
-  if (skipna) return exact ? go(ens_metrics_kernel<MP, true, true, 4>)
-                           : go(ens_metrics_kernel<MP, true, false, 4>);
-  return exact ? go(ens_metrics_kernel<MP, false, true, 4>)
-               : go(ens_metrics_kernel<MP, false, false, 4>);
+  if (skipna) return exact ? go(ens_metrics_kernel<MP, true, true>)
+                           : go(ens_metrics_kernel<MP, true, false>);
+  return exact ? go(ens_metrics_kernel<MP, false, true>)
+               : go(ens_metrics_kernel<MP, false, false>);
 }
 
 }  // namespace wb2

@@ -34,7 +34,6 @@ namespace rgt {
 
 constexpr int kThreads = 256;
 constexpr int kMaxGroup = 4;  // target longitudes per work item (template G <= this)
-constexpr int kTapBlock = 8;  // taps fetched together (their loads are all in flight)
 constexpr int kMaxDpt = 4;   // source latitudes per thread
 constexpr int kMaxSpans = 2;
 
@@ -368,11 +367,9 @@ int regrid_tma_try(wb2_ctx* ctx, const float* src, float* dst, int64_t nfield,
                    const wb2_csr* lat_w) {
   const char* force = getenv("WB2_REGRID_PATH");
   if (force && strcmp(force, "ldg") == 0) return 0;
-  const char* grp = getenv("WB2_REGRID_GROUP");  // experiments: targets per item
-  int rc = 0;
-  if (!(grp && grp[0] == '4'))
-    rc = regrid_tma_launch<2>(ctx, src, dst, nfield, src_field_stride, dst_field_stride, lon_w,
-                              lat_w);
+  // two targets per item; four when the two-target layout does not fit its shared memory
+  int rc = regrid_tma_launch<2>(ctx, src, dst, nfield, src_field_stride, dst_field_stride, lon_w,
+                                lat_w);
   if (rc == 0)
     rc = regrid_tma_launch<4>(ctx, src, dst, nfield, src_field_stride, dst_field_stride, lon_w,
                               lat_w);

@@ -39,9 +39,10 @@
 // Work decomposition: a work item = G row pairs (2 G rows) of one field; a job
 // = the items that share accumulators (mode 0: one item; mode 1: the same rows
 // of every time step of a slot; mode 2: a chunk of row groups of every time
-// step of a slot).  Persistent CTAs (2 per SM) take jobs round-robin; the
-// accumulators are flushed through shared memory (coalesced stores) at the end
-// of a job.  Deterministic: no atomics, fixed summation order.
+// step of a slot).  Persistent CTAs (the plan's MINB per SM) take jobs
+// round-robin; the accumulators are flushed through shared memory (coalesced
+// stores) at the end of a job.  Deterministic: no atomics, fixed summation
+// order.
 //
 // Shared-memory traffic per row: one staging read, three in-place passes over
 // the work array and the post twiddles.
@@ -262,16 +263,9 @@ constexpr int idem(int n2, int r) {  // CRT idempotent: 1 mod r, 0 mod n2 / r
   return x % n2;
 }
 
-// TWG_: read the split twiddles from global memory (L1) instead of a per-CTA
-// shared copy -- 11.5 KB less shared memory per CTA, which is what a fourth CTA
-// per SM needs.
-// DW_: two work buffers, alternating between items: stage A of item i + 1 may
-// then start while slower warps are still in stage C of item i (one CTA
-// barrier per item less, and a natural overlap of the two 5-warp stages).
-template <int RA_, int RB_, int RC_, int G_, int NT_, int MINB_ = 2, int TWG_ = 0, int DW_ = 0>
+template <int RA_, int RB_, int RC_, int G_, int NT_, int MINB_ = 2>
 struct Plan {
   static constexpr int RA = RA_, RB = RB_, RC = RC_, G = G_, NT = NT_, MINB = MINB_;
-  static constexpr int TWG = TWG_, DW = DW_;
   static constexpr int N2 = RA * RB * RC, NK = N2 + 1, N = 2 * N2;
   static constexpr int SA = N2 / RA, SB = N2 / RB, SC = N2 / RC;  // Good's input map
   static constexpr int EA = idem(N2, RA), EB = idem(N2, RB), EC = idem(N2, RC);
@@ -284,10 +278,9 @@ struct Plan {
   static constexpr int kRowBytes = N * 4;
   static constexpr int kStageBytes = 2 * G * kRowBytes;
   static constexpr int kWorkBytes = G * N2 * 16;
-  static constexpr int kTwnBytes = TWG ? 0 : N2 * 16;
+  static constexpr int kTwnBytes = N2 * 16;
   static constexpr int kTaskBytes = ((NTC * 16 + 127) / 128) * 128;
-  static constexpr int kWorkAll = (DW ? 2 : 1) * kWorkBytes;
-  static constexpr int kSmem = kStageBytes + kWorkAll + kTwnBytes + kTaskBytes + 64;
+  static constexpr int kSmem = kStageBytes + kWorkBytes + kTwnBytes + kTaskBytes + 64;
   // thread slots per row pair, padded to half-warps so that the 64-bit shared
   // accesses of a half-warp stay inside one row pair (conflict-free strides)
   static constexpr int PTB = (NTB + 15) / 16 * 16, PTC = (NTC + 15) / 16 * 16;
@@ -365,26 +358,21 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
   // in-place work array, planar: re and im as separate 64-bit planes (an
   // interleaved 128-bit element would need its four registers adjacent, which
   // costs four MOVs per store)
-  u64* work_re = reinterpret_cast<u64*>(smem + P::kStageBytes);
-  u64* work_im = work_re + G * N2;
-  u64* const work_base = work_re;
+  u64* const work_re = reinterpret_cast<u64*>(smem + P::kStageBytes);
+  u64* const work_im = work_re + G * N2;
   const ulonglong2* twn =
-      P::TWG ? reinterpret_cast<const ulonglong2*>(p.twn)
-             : reinterpret_cast<const ulonglong2*>(smem + P::kStageBytes + P::kWorkAll);
-  const int4* ctask = reinterpret_cast<const int4*>(smem + P::kStageBytes + P::kWorkAll +
+      reinterpret_cast<const ulonglong2*>(smem + P::kStageBytes + P::kWorkBytes);
+  const int4* ctask = reinterpret_cast<const int4*>(smem + P::kStageBytes + P::kWorkBytes +
                                                      P::kTwnBytes);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::kStageBytes + P::kWorkAll +
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::kStageBytes + P::kWorkBytes +
                                                P::kTwnBytes + P::kTaskBytes);
-  float* tile = reinterpret_cast<float*>(work_re);  // flush tile [2 G][NK], aliases `work`
-  uint32_t wsel = 0;  // DW: which work buffer the current item uses
+  float* const tile = reinterpret_cast<float*>(work_re);  // flush tile [2 G][NK], aliases `work`
   const int tid = threadIdx.x;
 
   {
-    if (!P::TWG) {
-      float4* d = reinterpret_cast<float4*>(smem + P::kStageBytes + P::kWorkAll);
-      for (int i = tid; i < N2; i += NT) d[i] = p.twn[i];
-    }
-    int4* t = reinterpret_cast<int4*>(smem + P::kStageBytes + P::kWorkAll + P::kTwnBytes);
+    float4* d = reinterpret_cast<float4*>(smem + P::kStageBytes + P::kWorkBytes);
+    for (int i = tid; i < N2; i += NT) d[i] = p.twn[i];
+    int4* t = reinterpret_cast<int4*>(smem + P::kStageBytes + P::kWorkBytes + P::kTwnBytes);
     for (int i = tid; i < P::NTC; i += NT) t[i] = p.ctask[i];
   }
   Cursor cur;
@@ -435,12 +423,6 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
   while (cur.valid(p)) {
     Cursor nxt = cur;
     nxt.advance(p);
-    if (P::DW) {
-      work_re = work_base + wsel * (P::kWorkBytes / 8);
-      work_im = work_re + G * N2;
-      tile = reinterpret_cast<float*>(work_re);
-      wsel ^= 1u;
-    }
     mbar_wait(full, parity);
     parity ^= 1u;
 
@@ -586,279 +568,8 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
         }
       }
     }
-    // one work buffer: it (and the tile in it) is overwritten by the next stage
-    // A; two: the next item writes the other one, and the one after that is
-    // behind the two barriers of the next item
-    if (!P::DW) __syncthreads();
+    __syncthreads();  // the work buffer (and the tile in it) is overwritten by the next stage A
     cur = nxt;
-  }
-}
-
-// ---------------------------------------------------------------------------
-// Warp-specialised variant.  The kernel above runs the three stages one after
-// the other behind CTA-wide barriers, where warps wait because stage B has
-// work for only 3 of the 5 warps and the TMA wait idles everyone.  Here the stages are THREE WARP
-// GROUPS of one persistent CTA per SM that work on different items at the same
-// time and hand buffers over through mbarriers:
-//     TMA -> staging[2] -> group A (radix RA) -> work[3] -> group B (radix RB,
-//     in place) -> group C (radix RC on mirrored pairs, split, power, accumulate)
-// Group sizes follow the per-item instruction counts (5 : 3 : 5 warps for
-// 720 = 9 * 16 * 5), so every group is busy all the time and the pipes see A's
-// shared-memory traffic, B's FADDs and C's mixed work interleaved.  Within a
-// group: a named barrier (bar.sync id, nthreads); between groups: mbarrier
-// arrive (release) by one elected thread after the group's barrier, try_wait
-// (acquire) by the consumers.
-// ---------------------------------------------------------------------------
-template <class P>
-struct WsLayout {
-  static constexpr int NSTG = 2, NWRK = 3;
-  static constexpr int WA = (P::G * P::NTA + 31) / 32, WB = (P::G * P::PTB + 31) / 32,
-                       WC = (P::G * P::PTC + 31) / 32;
-  static constexpr int NT = 32 * (WA + WB + WC);
-  static constexpr int kTileBytes = ((2 * P::G * P::NK * 4 + 127) / 128) * 128;
-  static constexpr int kOffWork = NSTG * P::kStageBytes;
-  static constexpr int kOffTwn = kOffWork + NWRK * P::kWorkBytes;
-  static constexpr int kOffTask = kOffTwn + P::kTwnBytes;
-  static constexpr int kOffTile = kOffTask + P::kTaskBytes;
-  static constexpr int kOffBar = kOffTile + kTileBytes;
-  static constexpr int kSmem = kOffBar + 128;
-};
-
-__device__ __forceinline__ void group_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-template <class P, int MODE>
-__global__ void __launch_bounds__(WsLayout<P>::NT, 1) spectrum_pfa_ws_kernel(const Params p) {
-  using L = WsLayout<P>;
-  constexpr int RA = P::RA, RB = P::RB, RC = P::RC, G = P::G;
-  constexpr int N2 = P::N2, NK = P::NK;
-  constexpr int NTA_T = 32 * L::WA, NTB_T = 32 * L::WB, NTC_T = 32 * L::WC;
-  extern __shared__ __align__(128) unsigned char smem[];
-  const ulonglong2* twn = reinterpret_cast<const ulonglong2*>(smem + L::kOffTwn);
-  const int4* ctask = reinterpret_cast<const int4*>(smem + L::kOffTask);
-  float* tile = reinterpret_cast<float*>(smem + L::kOffTile);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBar);
-  uint64_t* stg_full = bars;                  // [NSTG]  TMA landed
-  uint64_t* ab_full = bars + L::NSTG;         // [NWRK]  stage A wrote work[w]
-  uint64_t* bc_full = ab_full + L::NWRK;      // [NWRK]  stage B finished work[w]
-  uint64_t* w_empty = bc_full + L::NWRK;      // [NWRK]  stage C has read work[w]
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-
-  {
-    float4* d = reinterpret_cast<float4*>(smem + L::kOffTwn);
-    for (int i = tid; i < N2; i += L::NT) d[i] = p.twn[i];
-    int4* t = reinterpret_cast<int4*>(smem + L::kOffTask);
-    for (int i = tid; i < P::NTC; i += L::NT) t[i] = p.ctask[i];
-  }
-  if (tid == 0) {
-    for (int i = 0; i < L::NSTG + 3 * L::NWRK; ++i) mbar_init(bars + i, 1);
-    mbar_fence_init();
-  }
-  __syncthreads();
-
-  Cursor cur;
-  cur.job = blockIdx.x;
-  cur.open(p);
-
-  if (warp < L::WA) {
-    // ===================== group A: staging -> work (radix RA) =================
-    const int t = tid;
-    const bool on = t < G * P::NTA;
-    const int g = t / P::NTA, r = t - g * P::NTA;
-    const int nC = r / RB, nB = r - nC * RB;
-    const int e0 = (P::SB * nB + P::SC * nC) % N2;
-    const int src0 = 2 * g * N2, dst0 = g * N2 + nB * P::LB + nC;
-    Cursor pre = cur;  // the item whose rows are fetched next
-    if (t == 0) {
-      for (int k = 0; k < L::NSTG && pre.valid(p); ++k) {
-        issue_item<P>(p, pre, reinterpret_cast<float*>(smem + k * P::kStageBytes), &stg_full[k]);
-        pre.advance(p);
-      }
-    } else {
-      for (int k = 0; k < L::NSTG && pre.valid(p); ++k) pre.advance(p);
-    }
-    for (uint32_t it = 0; cur.valid(p); ++it, cur.advance(p)) {
-      const int s = it % L::NSTG, w = it % L::NWRK;
-      mbar_wait(&stg_full[s], (it / L::NSTG) & 1u);
-      mbar_wait(&w_empty[w], ((it / L::NWRK) & 1u) ^ 1u);
-      if (on) {
-        const float2* ra = reinterpret_cast<const float2*>(smem + s * P::kStageBytes) + src0;
-        const float2* rb = ra + N2;
-        u64* wre = reinterpret_cast<u64*>(smem + L::kOffWork + w * P::kWorkBytes);
-        u64* wim = wre + G * N2;
-        C2 v[RA];
-#pragma unroll
-        for (int nA = 0; nA < RA; ++nA) {
-          int e = e0 + P::SA * nA;
-          e = e >= N2 ? e - N2 : e;
-          const float2 a = ra[e], b = rb[e];
-          v[nA].re = pk2v(a.x, b.x);
-          v[nA].im = pk2v(a.y, b.y);
-        }
-        dft<RA>(v);
-#pragma unroll
-        for (int kA = 0; kA < RA; ++kA) {
-          wre[dst0 + kA * P::LA] = v[kA].re;
-          wim[dst0 + kA * P::LA] = v[kA].im;
-        }
-      }
-      group_sync(1, NTA_T);
-      if (t == 0) {
-        mbar_arrive(&ab_full[w]);
-        if (pre.valid(p))  // staging[s] is free again: fetch item it + NSTG into it
-          issue_item<P>(p, pre, reinterpret_cast<float*>(smem + s * P::kStageBytes), &stg_full[s]);
-      }
-      if (pre.valid(p)) pre.advance(p);
-    }
-  } else if (warp < L::WA + L::WB) {
-    // ===================== group B: radix RB, in place =========================
-    const int t = tid - NTA_T;
-    const int g = t / P::PTB, r = t - g * P::PTB;
-    const bool on = g < G && r < P::NTB;
-    const int off = g * N2 + r;
-    for (uint32_t it = 0; cur.valid(p); ++it, cur.advance(p)) {
-      const int w = it % L::NWRK;
-      mbar_wait(&ab_full[w], (it / L::NWRK) & 1u);
-      if (on) {
-        u64* wre = reinterpret_cast<u64*>(smem + L::kOffWork + w * P::kWorkBytes);
-        u64* wim = wre + G * N2;
-        C2 v[RB];
-#pragma unroll
-        for (int nB = 0; nB < RB; ++nB) v[nB] = {wre[off + nB * P::LB], wim[off + nB * P::LB]};
-        dft<RB>(v);
-#pragma unroll
-        for (int kB = 0; kB < RB; ++kB) {
-          wre[off + kB * P::LB] = v[kB].re;
-          wim[off + kB * P::LB] = v[kB].im;
-        }
-      }
-      group_sync(2, NTB_T);
-      if (t == 0) mbar_arrive(&bc_full[w]);
-    }
-  } else {
-    // ========== group C: radix RC on mirrored pairs, split, power, flush =======
-    const int t = tid - NTA_T - NTB_T;
-    const int c_g = t / P::PTC;
-    const bool on = c_g < G && t - c_g * P::PTC < P::NTC;
-    int c_off1 = 0, c_off2 = 0, c_k0 = 0, c_self = 0;
-    if (on) {
-      const int4 q = ctask[t - c_g * P::PTC];
-      c_off1 = c_g * N2 + q.x;
-      c_off2 = c_g * N2 + q.y;
-      c_k0 = q.z;
-      c_self = q.w;
-    }
-    u64 acc_a[RC], acc_b[RC];
-#pragma unroll
-    for (int i = 0; i < RC; ++i) acc_a[i] = acc_b[i] = 0ull;
-    for (uint32_t it = 0; cur.valid(p); ++it, cur.advance(p)) {
-      const int w = it % L::NWRK;
-      mbar_wait(&bc_full[w], (it / L::NWRK) & 1u);
-      C2 b1[RC], b2[RC];
-      if (on) {
-        const u64* wre = reinterpret_cast<const u64*>(smem + L::kOffWork + w * P::kWorkBytes);
-        const u64* wim = wre + G * N2;
-#pragma unroll
-        for (int i = 0; i < RC; ++i) {
-          b1[i] = {wre[c_off1 + i], wim[c_off1 + i]};
-          b2[i] = {wre[c_off2 + i], wim[c_off2 + i]};
-        }
-      }
-      group_sync(3, NTC_T);  // everyone has its values: the buffer can go back to A
-      if (t == 0) mbar_arrive(&w_empty[w]);
-      if (on) {
-        dft<RC>(b1);
-        dft<RC>(b2);
-        u64 scl = 0ull;
-        if (MODE == 2) {
-          const int row = 2 * (G * cur.gi + c_g);
-          scl = pk2(__ldg(p.scale + row), __ldg(p.scale + row + 1));
-        }
-#pragma unroll
-        for (int kC = 0; kC < RC; ++kC) {
-          int pbin = c_k0 + (kC * P::EC) % N2;
-          pbin = pbin >= N2 ? pbin - N2 : pbin;
-          const ulonglong2 wv = twn[pbin];  // (wr, wr), (wi, wi)
-          const C2 zp = b1[kC], zq = b2[(RC - kC) % RC];
-          const u64 e_re = add2(zp.re, zq.re), e_im = sub2(zp.im, zq.im);
-          const u64 d_re = sub2(zp.re, zq.re), d_im = add2(zp.im, zq.im);
-          const u64 t1 = fma2(wv.y, d_re, mul2(wv.x, d_im));
-          const u64 t2 = sub2(mul2(wv.x, d_re), mul2(wv.y, d_im));
-          const u64 xa_re = add2(e_re, t1), xa_im = sub2(e_im, t2);
-          const u64 xb_re = sub2(e_re, t1), xb_im = add2(e_im, t2);
-          if (MODE == 2) {
-            const u64 pa = fma2(xa_im, xa_im, mul2(xa_re, xa_re));
-            const u64 pb = fma2(xb_im, xb_im, mul2(xb_re, xb_re));
-            acc_a[kC] = fma2(pa, scl, acc_a[kC]);
-            acc_b[kC] = fma2(pb, scl, acc_b[kC]);
-          } else {
-            acc_a[kC] = fma2(xa_im, xa_im, fma2(xa_re, xa_re, acc_a[kC]));
-            acc_b[kC] = fma2(xb_im, xb_im, fma2(xb_re, xb_re, acc_b[kC]));
-          }
-        }
-      }
-      if (cur.last_of_job(p)) {
-        // the flush tile is private to this group
-        if (on) {
-          float* ta = tile + (2 * c_g) * NK;
-          float* tb = ta + NK;
-          float sa = 1.f, sb = 1.f;
-          if (MODE != 2) {
-            const int row = 2 * (G * cur.gi + c_g);
-            sa = __ldg(p.scale + row);
-            sb = __ldg(p.scale + row + 1);
-          }
-#pragma unroll
-          for (int kC = 0; kC < RC; ++kC) {
-            int pbin = c_k0 + (kC * P::EC) % N2;
-            pbin = pbin >= N2 ? pbin - N2 : pbin;
-            const bool va = !c_self || kC <= (RC - kC) % RC;
-            const bool vb = va && (2 * pbin != N2);
-            const float h0 = pbin == 0 ? 0.5f : 1.f;
-            if (va) {
-              ta[pbin] = lo2(acc_a[kC]) * (sa * h0);
-              tb[pbin] = hi2(acc_a[kC]) * (sb * h0);
-            }
-            if (vb) {
-              ta[N2 - pbin] = lo2(acc_b[kC]) * sa;
-              tb[N2 - pbin] = hi2(acc_b[kC]) * sb;
-            }
-            acc_a[kC] = acc_b[kC] = 0ull;
-          }
-        }
-        group_sync(3, NTC_T);
-        if (MODE == 2) {
-          float* o = p.out + cur.job * NK;
-          for (int k = t; k < NK; k += NTC_T) {
-            float sum = 0.f;
-#pragma unroll
-            for (int rr = 0; rr < 2 * G; ++rr) sum += tile[rr * NK + k];
-            o[k] = sum;
-          }
-        } else {
-          const int row0 = 2 * G * cur.gi;
-          const int n = min(2 * G, p.nrow - row0) * NK;
-          float* o = p.out + (cur.slot * p.nrow + row0) * int64_t(NK);
-          constexpr int kU = 6;
-          for (int i0 = t; i0 < n; i0 += kU * NTC_T) {
-            float v[kU];
-#pragma unroll
-            for (int u = 0; u < kU; ++u) {
-              const int i = i0 + u * NTC_T;
-              v[u] = (MODE == 1 && i < n) ? o[i] : 0.f;
-            }
-#pragma unroll
-            for (int u = 0; u < kU; ++u) {
-              const int i = i0 + u * NTC_T;
-              if (i < n) o[i] = v[u] + tile[i];
-            }
-          }
-        }
-        group_sync(3, NTC_T);  // the tile is reused by the next job
-      }
-    }
   }
 }
 
@@ -903,7 +614,7 @@ static void build_tables(std::vector<float4>* twn, std::vector<int4>* ctask) {
     }
 }
 
-template <class P, bool warp_specialised = false>
+template <class P>
 static int launch(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t nrow,
                   const double* scale, float* out, int mode, int64_t nslot) {
   const int latsum_accumulate = mode == 3;  // mode 3 = mode 2 adding to `out`
@@ -924,7 +635,7 @@ static int launch(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t nrow,
   p.ngroup = (npair + P::G - 1) / P::G;
   p.mode = mode;
   // latitude chunks of mode 2: enough jobs to fill the machine, few partials
-  const int64_t want_jobs = int64_t(ctx->num_sms) * (warp_specialised ? 1 : P::MINB) * 4;
+  const int64_t want_jobs = int64_t(ctx->num_sms) * P::MINB * 4;
   if (mode == 2) {
     int nchunk = static_cast<int>((want_jobs + nslot - 1) / nslot);
     if (nchunk < 1) nchunk = 1;
@@ -954,25 +665,13 @@ static int launch(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t nrow,
   p.scale = pk.dev<float>(o3);
   p.out = mode == 2 ? pk.dev<float>(o4) : out;
 
-  if constexpr (warp_specialised) {
-    using L = WsLayout<P>;
-    const int64_t max_cta = ctx->num_sms;  // one persistent CTA per SM
-    const unsigned grid = static_cast<unsigned>(p.njob < max_cta ? p.njob : max_cta);
-    auto kernel = mode == 0 ? spectrum_pfa_ws_kernel<P, 0>
-                            : (mode == 1 ? spectrum_pfa_ws_kernel<P, 1>
-                                         : spectrum_pfa_ws_kernel<P, 2>);
-    WB2_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      L::kSmem));
-    kernel<<<grid, L::NT, L::kSmem, ctx->stream>>>(p);
-  } else {
-    const int64_t max_cta = int64_t(ctx->num_sms) * P::MINB;
-    const unsigned grid = static_cast<unsigned>(p.njob < max_cta ? p.njob : max_cta);
-    auto kernel = mode == 0 ? spectrum_pfa_kernel<P, 0>
-                            : (mode == 1 ? spectrum_pfa_kernel<P, 1> : spectrum_pfa_kernel<P, 2>);
-    WB2_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      P::kSmem));
-    kernel<<<grid, P::NT, P::kSmem, ctx->stream>>>(p);
-  }
+  const int64_t max_cta = int64_t(ctx->num_sms) * P::MINB;
+  const unsigned grid = static_cast<unsigned>(p.njob < max_cta ? p.njob : max_cta);
+  auto kernel = mode == 0 ? spectrum_pfa_kernel<P, 0>
+                          : (mode == 1 ? spectrum_pfa_kernel<P, 1> : spectrum_pfa_kernel<P, 2>);
+  WB2_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    P::kSmem));
+  kernel<<<grid, P::NT, P::kSmem, ctx->stream>>>(p);
   WB2_CUDA_TRY(cudaGetLastError());
   ctx->launches += 1;
   if (mode == 2) {
@@ -1002,28 +701,9 @@ int spectrum_pfa_try(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t nrow,
   if (nrow < 1 || nfield < 1 || nslot < 1 || nfield % nslot != 0) return 0;
   int rc;
   switch (ncol) {
-    case 1440: {
-      const char* plan = getenv("WB2_PFA_PLAN");  // experiments: CTA shape
-      if (plan && plan[0] == 'w')  // warp-specialised pipeline, one CTA per SM
-        rc = pfa::launch<pfa::Plan<9, 16, 5, 2, 160, 3>, true>(ctx, x, nfield, nrow, scale, out,
-                                                               mode, nslot);
-      else if (plan && plan[0] == '4')  // 4 CTAs per SM (102 registers, twiddles via L1)
-        rc = pfa::launch<pfa::Plan<9, 16, 5, 2, 160, 4, 1>>(ctx, x, nfield, nrow, scale, out,
-                                                            mode, nslot);
-      else if (plan && plan[0] == '0')
-        rc = pfa::launch<pfa::Plan<9, 16, 5, 3, 256, 2>>(ctx, x, nfield, nrow, scale, out, mode,
-                                                         nslot);
-      else if (plan && plan[0] == '2')
-        rc = pfa::launch<pfa::Plan<9, 16, 5, 1, 96, 5>>(ctx, x, nfield, nrow, scale, out, mode,
-                                                        nslot);
-      else if (plan && plan[0] == 'd')  // double work buffer, 3 CTAs, twiddles via L1
-        rc = pfa::launch<pfa::Plan<9, 16, 5, 2, 160, 3, 1, 1>>(ctx, x, nfield, nrow, scale, out,
-                                                               mode, nslot);
-      else  // 3 CTAs of 5 warps per SM: fastest on H100 in every mode (DESIGN.md, K4)
-        rc = pfa::launch<pfa::Plan<9, 16, 5, 2, 160, 3>>(ctx, x, nfield, nrow, scale, out, mode,
-                                                         nslot);
-      break;
-    }
+    // 3 CTAs of 5 warps per SM: fastest on H100 in every mode (DESIGN.md, K4)
+    case 1440: rc = pfa::launch<pfa::Plan<9, 16, 5, 2, 160, 3>>(ctx, x, nfield, nrow, scale, out,
+                                                                 mode, nslot); break;
     case 720: rc = pfa::launch<pfa::Plan<9, 8, 5, 5, 256>>(ctx, x, nfield, nrow, scale, out,
                                                             mode, nslot); break;
     case 240: rc = pfa::launch<pfa::Plan<3, 8, 5, 6, 256>>(ctx, x, nfield, nrow, scale, out,
