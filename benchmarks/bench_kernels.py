@@ -14,6 +14,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel resample --steps 5
   python benchmarks/bench_kernels.py --kernel wind_dynamics --steps 20
   python benchmarks/bench_kernels.py --kernel precip_accumulation --steps 20
+  python benchmarks/bench_kernels.py --kernel column_integral --steps 20
   python benchmarks/bench_kernels.py --kernel quantile --steps 5
   python benchmarks/bench_kernels.py --kernel average --steps 5
 """
@@ -625,6 +626,59 @@ def bench_wind_dynamics(args):
          'cells', dict(card))
 
 
+def bench_column_integral(args):
+  """Device-resident 0.25-degree (time=4, level=37, 721, 1440) float32 q, u, v:
+  integrated vapor transport over 300-1000 hPa (20 of the 37 levels: 3 x 4 B
+  read per selected level and cell, 4 B written per cell) and eddy kinetic
+  energy over all 37 levels (2 x 4 B read per level and cell, 4 B written) in
+  both layouts, next to a device copy of q measured in the same run; all of it
+  twice."""
+  torch, _lib, ctx = setup()
+  from weatherbench2_b200 import _derived_column as dc
+  card = _card()
+  level = np.array([1, 2, 3, 5, 7, 10, 20, 30, 50, 70, 100, 125, 150, 175,
+                    200, 225, 250, 300, 350, 400, 450, 500, 550, 600, 650,
+                    700, 750, 775, 800, 825, 850, 875, 900, 925, 950, 975,
+                    1000])
+  nouter, nlev, ncell = 4, level.size, NLAT * NLON
+  shape = (nouter, nlev, NLAT, NLON)
+  gen = torch.Generator(device='cuda').manual_seed(0)
+  q = torch.empty(shape, device='cuda').uniform_(0, 0.02, generator=gen)
+  u = torch.empty(shape, device='cuda').normal_(5, 12, generator=gen)
+  v = torch.empty(shape, device='cuda').normal_(0, 8, generator=gen)
+  out = torch.empty((nouter, NLAT, NLON), device='cuda')
+  lev0 = int(np.searchsorted(level, 300))
+  nsel = nlev - lev0
+  off = lev0 * ncell * 4
+  w_ivt = dc.level_weights(level[lev0:])
+  w_all = dc.level_weights(level)
+  cases = [
+      ('IVT 300-1000 hPa (20 levels)', nsel * 12 + 4,
+       lambda: ctx.column_integral(
+           dc.IVT, _lib.F32, q.data_ptr() + off, u.data_ptr() + off,
+           v.data_ptr() + off, nouter, nlev * ncell, nsel, ncell, 0, 0, w_ivt,
+           out.data_ptr())),
+      ('EKE (latitude, longitude)', nlev * 8 + 4,
+       lambda: ctx.column_integral(
+           dc.EKE, _lib.F32, None, u.data_ptr(), v.data_ptr(), nouter,
+           nlev * ncell, nlev, ncell, NLON, 1, w_all, out.data_ptr())),
+      ('EKE (longitude, latitude)', nlev * 8 + 4,
+       lambda: ctx.column_integral(
+           dc.EKE, _lib.F32, None, u.data_ptr(), v.data_ptr(), nouter,
+           nlev * ncell, nlev, ncell, NLON, NLAT, w_all, out.data_ptr())),
+  ]
+  copy = torch.empty_like(q)
+  for run in (1, 2):  # twice in one process, to show the spread
+    for name, per_cell, fn in cases:
+      ms = timeit(fn, args.steps)
+      report(f'column_integral {name} 4x37x721x1440', ms,
+             nouter * ncell * per_cell, nouter * ncell, 'columns',
+             dict(card, run=run))
+    ms = timeit(lambda: copy.copy_(q), args.steps)
+    report('device copy 4x37x721x1440 (torch copy_)', ms, q.numel() * 8,
+           q.numel(), 'cells', dict(card, run=run))
+
+
 def precip_bytes(nouter, ntime, ninner, window, esize=4, block=256):
   """Bytes a precipitation accumulation needs: the input read once plus the
   `window` halo rows each block of `block` outputs stages again, and the
@@ -900,7 +954,7 @@ if __name__ == '__main__':
                            'maps', 'threshold', 'climatology',
                            'climatology_quantile', 'resample',
                            'wind_dynamics', 'precip_accumulation',
-                           'quantile', 'average'])
+                           'column_integral', 'quantile', 'average'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -913,5 +967,6 @@ if __name__ == '__main__':
    'resample': bench_resample,
    'wind_dynamics': bench_wind_dynamics,
    'precip_accumulation': bench_precip_accumulation,
+   'column_integral': bench_column_integral,
    'quantile': bench_quantile,
    'average': bench_average}[a.kernel](a)

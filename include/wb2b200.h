@@ -334,6 +334,62 @@ int wb2_wind_dynamics(wb2_ctx* ctx, int kind, const float* u, const float* v,
                       const double* cos_lat, const double* coriolis,
                       const double* pressure, float* out);
 
+/* wb2_column_integral replaces the level integrals of derived_variables.py:
+ * TotalColumnWater.compute (:383-385), IntegratedWaterTransport.compute (:418-430)
+ * and EddyKineticEnergy.compute (:223-228), all of which end in xarray's
+ * integrate('level') = sum(dx * 0.5 * (y[1:] + y[:-1]), skipna=False):      */
+#define WB2_COL_TOTAL_COLUMN 0 /* (1/9.81) * S(q)                                   */
+#define WB2_COL_IVT 1          /* (1/9.81) * sqrt(S(q*u)^2 + S(q*v)^2)               */
+#define WB2_COL_EKE 2          /* 0.5 * S(u'^2 + v'^2), u' = u - zonal mean of u      */
+/* q, u, v   device arrays of `dtype` (WB2_F32 / WB2_F64) [nouter][nlev][ninner]
+ *           with outer_stride elements between outer indices (>= nlev * ninner;
+ *           larger when the levels are a contiguous window of a longer axis,
+ *           the pointers then start at the window's first level).  Kind 0 reads
+ *           q, kind 1 q, u and v, kind 2 u and v; an operand a kind does not
+ *           read may be NULL.
+ *   nlon, lon_stride  kind 2 only (ignored otherwise): a level of ninner cells is
+ *           nrow = ninner / nlon rows of nlon longitudes, with lon_stride 1
+ *           ([nrow][nlon]) or nrow ([nlon][nrow]);
+ *   weight  host [nlev - 1] float64, w_k = 0.5 * (level[k+1] - level[k]) with
+ *           the level coordinate taken as float64 (may be NULL when nlev < 2);
+ *   out     device [nouter][ninner] of `dtype`, the inner cells in the inputs'
+ *           order.
+ * Kind 2 with lon_stride 1 runs one CTA per row; with lon_stride nrow, one CTA
+ * per tile of up to 8 adjacent rows, so that a warp reads adjacent rows.  Both
+ * keep the level sums of their cells in shared memory: nlon * (16 + 2 *
+ * sizeof(T)) bytes per CTA for lon_stride 1, tile * nlon * 16 for lon_stride
+ * nrow (the tile shrinks to fit, down to 1 row).
+ * Numerics, with T the data type and S(y) = sum_k w_k * f64(T(y[k] + y[k+1]))
+ * accumulated in float64 from k = 0 upward, starting from the k = 0 term:
+ *   kind 0  (1/9.81) * S(q), the double constant 1/9.81 times S (not S / 9.81);
+ *   kind 1  y = T(q * u) and T(q * v), rounded in T as the reference's q * u;
+ *           (1/9.81) * sqrt(Su^2 + Sv^2) in float64;
+ *   kind 2  y_k = u'^2 + v'^2 in float64, u' = f64(u) - ubar, ubar the mean of
+ *           the non-NaN cells of that level's row accumulated in float64 (NaN for
+ *           an all-NaN row); the pair sum y[k] + y[k+1] is float64 too; 0.5 * S.
+ * Correctly rounded operations only (no FMA contraction); the result is rounded
+ * once to T.  NaN propagates through the level sum (skipna=False); nlev < 2 gives
+ * 0, as trapz does.  Deviations from the reference:
+ *   kinds 0 and 1  only the summation order: where `level` is the innermost axis
+ *           NumPy sums the terms pairwise, so the float64 sums differ in the
+ *           last bits (|dS| <= nlev * 2^-53 * sum_k |w_k p_k|); in any other layout
+ *           the order is this one.  A float32 result is the reference's float64
+ *           result rounded once.
+ *   kind 2  the reference rounds ubar, u' and the squares to float32 and sums
+ *           ubar in float32; for float32 data the gap to it is at most
+ *           |dE| <= 0.5 * sum_k |w_k| (e_k + e_{k+1}), with maxima over level
+ *           k's row (NaN cells left out)
+ *           e_k = 2^-23 (5 max y + 2 nlon (max|u'| max|u| + max|v'| max|v|))
+ *           (DESIGN.md section 8h derives it).
+ * Float32 level coordinates are taken as float64.  Errors: NULL operands, negative
+ * sizes, an unknown kind or dtype, outer_stride < nlev * ninner, for kind 2 an
+ * ninner that is not a multiple of nlon, another lon_stride, or a row too wide for
+ * shared memory.  One kernel launch per call.                                   */
+int wb2_column_integral(wb2_ctx* ctx, int kind, int dtype, const void* q, const void* u,
+                        const void* v, int64_t nouter, int64_t outer_stride, int32_t nlev,
+                        int64_t ninner, int32_t nlon, int64_t lon_stride,
+                        const double* weight, void* out);
+
 /* wb2_ens_mean replaces the ensemble-mean pipeline of
  * scripts/compute_ensemble_mean.py:110-141 (xbeam.Mean(realization, skipna)):
  * out[field][cell] = mean_m x[off_x[field] + m * member_stride + cell], float32;

@@ -127,6 +127,9 @@ PROTOTYPES = {
         C.c_int64, C.c_int64, C.POINTER(C.c_double), C.c_int,
         C.POINTER(C.c_double), C.c_int, C.POINTER(C.c_double),
         C.POINTER(C.c_double), C.POINTER(C.c_double), _P]),
+    'wb2_column_integral': (C.c_int, [
+        _P, C.c_int, C.c_int, _P, _P, _P, C.c_int64, C.c_int64, C.c_int32,
+        C.c_int64, C.c_int32, C.c_int64, C.POINTER(C.c_double), _P]),
     'wb2_ens_mean': (C.c_int, [_P, _P, C.c_int32, C.c_int64, C.c_int64, _I64P,
                                C.c_int64, C.c_int, _P]),
     'wb2_spectrum_interp': (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32,
@@ -651,6 +654,21 @@ class Context:
         _as_ptr(cor, C.c_double), _as_ptr(pres, C.c_double),
         _P(out) if out else None))
     del tabs
+
+  def column_integral(self, kind: int, dtype: int, q: Optional[int],
+                      u: Optional[int], v: Optional[int], nouter: int,
+                      outer_stride: int, nlev: int, ninner: int, nlon: int,
+                      lon_stride: int, weight: Optional[np.ndarray], out: int):
+    """q / u / v / out are DEVICE addresses (wb2_column_integral); weight
+    is the host float64 table w_k = 0.5 * (level[k+1] - level[k])."""
+    w = (None if weight is None
+         else np.ascontiguousarray(weight, dtype=np.float64))
+    check(self.lib.wb2_column_integral(
+        self.handle, int(kind), int(dtype), *(_P(p) if p else None
+                                              for p in (q, u, v)),
+        int(nouter), int(outer_stride), int(nlev), int(ninner), int(nlon),
+        int(lon_stride), _as_ptr(w, C.c_double), _P(out) if out else None))
+    del w
 
   def ens_mean(self, x: int, nmember: int, member_stride: int,
                off_x: np.ndarray, slab: int, skipna: bool, out: int):

@@ -6,9 +6,12 @@ vorticity, vertical velocity and the geostrophic / ageostrophic winds -- live in
 _derived_wind.py (csrc/derived.cu, csrc/wind_dynamics.cu) and are re-exported
 here.  The precipitation accumulations of derived_variables.py:471-528 and
 685-720 live in _derived_precip.py (csrc/precip_accumulation.cu,
-csrc/resample.cu) and are re-exported here.  The remaining derived variables
-of the reference (eddy kinetic energy, lapse rate, column integrals, relative
-humidity) are not reproduced.
+csrc/resample.cu) and are re-exported here.  The column integrals over
+pressure level of derived_variables.py:212-228 and 365-430 -- eddy kinetic
+energy, total column water and integrated water transport -- live in
+_derived_column.py (csrc/column_integral.cu) and are re-exported here.  The
+remaining derived variables of the reference (lapse rate, relative humidity)
+are not reproduced.
 """
 from __future__ import annotations
 
@@ -302,14 +305,17 @@ from weatherbench2_b200._derived_wind import (  # noqa: E402  pylint: disable=wr
     _GeostrophicWindVariable)
 from weatherbench2_b200._derived_precip import (  # noqa: E402  pylint: disable=wrong-import-position
     AggregatePrecipitationAccumulation, PrecipitationAccumulation)
+from weatherbench2_b200._derived_column import (  # noqa: E402  pylint: disable=wrong-import-position
+    EddyKineticEnergy, IntegratedWaterTransport, TotalColumnWater)
 
 # The named derived variables of weatherbench2/derived_variables.py:724-773 that
 # have a device implementation: wind speed, the horizontal-derivative family
 # (divergence, vorticity, vertical velocity, geostrophic and ageostrophic
-# winds) and the precipitation accumulations.  The remaining entries of the
-# reference's table (eddy kinetic energy, lapse rate, column integrals,
-# relative humidity) are not reproduced; asking for one raises KeyError here
-# instead of silently running on the host.
+# winds), the column integrals (eddy kinetic energy, total column water,
+# integrated vapor transport) and the precipitation accumulations.  The
+# remaining entries of the reference's table (lapse rate, relative humidity)
+# are not reproduced; asking for one raises KeyError here instead of silently
+# running on the host.
 DERIVED_VARIABLE_DICT = {
     'wind_speed': WindSpeed(u_name='u_component_of_wind',
                             v_name='v_component_of_wind'),
@@ -318,12 +324,23 @@ DERIVED_VARIABLE_DICT = {
     'divergence': WindDivergence(),
     'vorticity': WindVorticity(),
     'vertical_velocity': VerticalVelocity(),
+    'eddy_kinetic_energy': EddyKineticEnergy(),
     'geostrophic_wind_speed': GeostrophicWindSpeed(),
     'u_component_of_geostrophic_wind': UComponentOfGeostrophicWind(),
     'v_component_of_geostrophic_wind': VComponentOfGeostrophicWind(),
     'ageostrophic_wind_speed': AgeostrophicWindSpeed(),
     'u_component_of_ageostrophic_wind': UComponentOfAgeostrophicWind(),
     'v_component_of_ageostrophic_wind': VComponentOfAgeostrophicWind(),
+    'total_column_vapor': TotalColumnWater(
+        water_species_name='specific_humidity'
+    ),
+    'total_column_liquid': TotalColumnWater(
+        water_species_name='specific_cloud_liquid_water_content'
+    ),
+    'total_column_ice': TotalColumnWater(
+        water_species_name='specific_cloud_ice_water_content'
+    ),
+    'integrated_vapor_transport': IntegratedWaterTransport(),
     'total_precipitation_6hr': PrecipitationAccumulation(
         total_precipitation_name='total_precipitation',
         accumulation_hours=6,
