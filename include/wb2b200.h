@@ -802,6 +802,11 @@ int wb2_regrid_bilinear(wb2_ctx* ctx, const float* src, float* dst,
  *          is ADDED to slot  i % nfield_out  (device-side time-sum for the
  *          script's `xbeam.Mean(['time'])`,
  *          scripts/compute_zonal_energy_spectrum.py:234)
+ * Each row is transformed as x - x[0] (x[0] added back to bin 0), so the
+ * float32 rounding scales with the row's variation, not its mean.  Per bin,
+ * with u = 2^-24, D = max|x_n - mean|, F_k the exact DFT of the float32 row:
+ *   |got_k - want_k| <= c_k scale (2 |F_k| e + e^2) + m u want_k,
+ *   e = C_plan u D,  C_plan = 2 L / sqrt(N / 2)  (DESIGN.md K4: L, m, bin 0).
  */
 int wb2_zonal_spectrum(wb2_ctx* ctx, const float* x, int64_t nfield,
                        int32_t nrow, int32_t ncol, const double* scale,
@@ -816,7 +821,8 @@ int wb2_zonal_spectrum(wb2_ctx* ctx, const float* x, int64_t nfield,
  * where S_ref is the spectrum WITHOUT the circumference factor, i.e. the caller
  * passes scale[row] = circumference(row) * w(row) with w the (normalised)
  * latitude weight of weatherbench2/metrics.py:40-60 (or a latitude-band mask
- * times it).  Fields are slot-minor like wb2_zonal_spectrum's accumulate mode
+ * times it; rows whose scale is 0 are skipped, so NaN / inf outside a band
+ * do not reach it).  Fields are slot-minor like wb2_zonal_spectrum's accumulate mode
  * (field i belongs to slot i % nfield_out), so a time mean is the same call.
  *   out    device [nfield_out][ncol/2+1] float32, overwritten
  * The per-latitude spectrum is never written: 4 B read per cell, ~0 written. */

@@ -33,6 +33,10 @@ namespace wb2 {
 constexpr int kSpThreads = 256;
 constexpr int kSpMaxStages = 16;
 constexpr int kSpMaxAcc = 24;
+constexpr int kSpMaxRows = 32;  // rows per CTA
+// static shared memory of the kernels (the per-row shifts): counts towards the
+// 48 KB a launch may use without opting in
+constexpr size_t kSpStaticSmem = kSpMaxRows * sizeof(float);
 
 struct SpecParams {
   const float* x;
@@ -62,6 +66,14 @@ __device__ __forceinline__ int pad(int i) { return i + (i >> 4); }
 // floor(x / d) for 0 <= x < 2^20 via multiply-high; m = ceil(2^32 / d)
 __device__ __forceinline__ int fast_div(int x, unsigned m, int d) {
   return d == 1 ? x : static_cast<int>(__umulhi(static_cast<unsigned>(x), m));
+}
+// The shift subtracted from a row before its transform: the row's first element
+// (0 when that is not finite: inf - inf would turn the row into NaN).  The DFT
+// is shift-invariant except for bin 0, so the butterflies round relative to
+// the row's variation instead of its mean; the post-pass adds N s back to X_0.
+__device__ __forceinline__ float row_shift(const float2* row) {
+  const float s = __ldg(reinterpret_cast<const float*>(row));
+  return isfinite(s) ? s : 0.f;
 }
 static unsigned magic(int d) {
   return d <= 1 ? 0u : static_cast<unsigned>(((1ull << 32) + d - 1) / d);
@@ -189,20 +201,27 @@ struct StageInfo {
 
 // One Stockham stage of radix R over `nrows` rows held in `src` (or read from
 // global memory when FROM_GLOBAL), writing `dst` (both padded, pitch `pitch`).
+// The first stage transforms x - s and records s per row in `shift`.
 template <int R, bool FROM_GLOBAL>
 __device__ __forceinline__ void stage(const float2* __restrict__ src, float2* __restrict__ dst,
                                       const float2* __restrict__ gsrc, int n2, int pitch,
                                       const float2* __restrict__ tw2, const StageInfo si,
-                                      int nrows) {
+                                      int nrows, float* shift) {
   const int total = nrows * si.t;
   for (int idx = threadIdx.x; idx < total; idx += kSpThreads) {
     const int row = fast_div(idx, si.m_t, si.t);
     const int j = idx - row * si.t;
     float2 v[R];
+    const float s = FROM_GLOBAL ? row_shift(gsrc + row * n2) : 0.f;
+    if (FROM_GLOBAL && j == 0) shift[row] = s;
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-      if (FROM_GLOBAL) v[r] = __ldcs(gsrc + row * n2 + j + r * si.t);
-      else v[r] = src[row * pitch + pad(j + r * si.t)];
+      if (FROM_GLOBAL) {
+        v[r] = __ldcs(gsrc + row * n2 + j + r * si.t);
+        v[r] = make_float2(__fsub_rn(v[r].x, s), __fsub_rn(v[r].y, s));
+      } else {
+        v[r] = src[row * pitch + pad(j + r * si.t)];
+      }
     }
     const int q = fast_div(j, si.m_ns, si.ns);
     const int k = j - q * si.ns;
@@ -221,16 +240,16 @@ __device__ __forceinline__ void stage(const float2* __restrict__ src, float2* __
 template <bool FROM_GLOBAL>
 __device__ __forceinline__ void run_stage(int r, const float2* src, float2* dst, const float2* g,
                                           int n2, int pitch, const float2* tw2,
-                                          const StageInfo si, int nrows) {
+                                          const StageInfo si, int nrows, float* shift) {
   switch (r) {
-    case 1: stage<1, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows); break;
-    case 2: stage<2, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows); break;
-    case 3: stage<3, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows); break;
-    case 4: stage<4, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows); break;
-    case 5: stage<5, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows); break;
-    case 8: stage<8, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows); break;
-    case 9: stage<9, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows); break;
-    default: stage<16, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows); break;
+    case 1: stage<1, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows, shift); break;
+    case 2: stage<2, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows, shift); break;
+    case 3: stage<3, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows, shift); break;
+    case 4: stage<4, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows, shift); break;
+    case 5: stage<5, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows, shift); break;
+    case 8: stage<8, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows, shift); break;
+    case 9: stage<9, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows, shift); break;
+    default: stage<16, FROM_GLOBAL>(src, dst, g, n2, pitch, tw2, si, nrows, shift); break;
   }
 }
 
@@ -240,6 +259,7 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_kernel(const SpecParams p
   float2* buf_b = buf_a + size_t(p.rows_per_block) * p.row_pitch;
   float2* tw2 = buf_b + size_t(p.rows_per_block) * p.row_pitch;
   float2* twn = tw2 + p.n2;
+  __shared__ float shift[kSpMaxRows];
 
   for (int i = threadIdx.x; i < p.n2; i += kSpThreads) tw2[i] = p.tw2[i];
   for (int i = threadIdx.x; i <= p.n2; i += kSpThreads) twn[i] = p.twn[i];
@@ -271,8 +291,8 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_kernel(const SpecParams p
       si.step = p.n2 / (ns * r);
       si.m_t = (unsigned)(((1ull << 32) + si.t - 1) / si.t);
       si.m_ns = (unsigned)(((1ull << 32) + ns - 1) / ns);
-      if (s == 0) run_stage<true>(r, src, dst, g, p.n2, p.row_pitch, tw2, si, nrows);
-      else run_stage<false>(r, src, dst, g, p.n2, p.row_pitch, tw2, si, nrows);
+      if (s == 0) run_stage<true>(r, src, dst, g, p.n2, p.row_pitch, tw2, si, nrows, shift);
+      else run_stage<false>(r, src, dst, g, p.n2, p.row_pitch, tw2, si, nrows, shift);
       __syncthreads();
       float2* tmp = src;
       src = dst;
@@ -293,7 +313,8 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_kernel(const SpecParams p
         const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y + zc.y));
         const float2 d = csub(zk, zc);
         const float2 o = make_float2(0.5f * d.y, -0.5f * d.x);
-        const float2 xk = cadd(e, cmul(twn[k], o));
+        float2 xk = cadd(e, cmul(twn[k], o));
+        if (k == 0) xk.x += float(p.n) * shift[row];
         const float pw = (xk.x * xk.x + xk.y * xk.y) * (k == 0 ? 1.f : 2.f) * p.scale[row0 + row];
         acc[it] += pw;
       }
@@ -318,10 +339,12 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_kernel(const SpecParams p
 // both loads and the complex product W_N^k * O):
 //     X_k = E + W O,   X_{N2-k} = conj(E - W O).
 // ---------------------------------------------------------------------------
+// The first stage (FROM_GLOBAL) transforms x - s and records s per row in `shift`.
 template <int R, int NS, int N2, bool FROM_GLOBAL>
 __device__ __forceinline__ void stage_ct(const float2* __restrict__ src, float2* __restrict__ dst,
                                          const float2* __restrict__ gsrc,
-                                         const float2* __restrict__ tw2, int nrows) {
+                                         const float2* __restrict__ tw2, int nrows,
+                                         float* shift) {
   constexpr int T = N2 / R;
   constexpr int STEP = N2 / (NS * R);
   constexpr int PITCH = N2 + (N2 >> 4) + 1;
@@ -330,10 +353,16 @@ __device__ __forceinline__ void stage_ct(const float2* __restrict__ src, float2*
     const int row = idx / T;
     const int j = idx - row * T;
     float2 v[R];
+    const float s = FROM_GLOBAL ? row_shift(gsrc + row * N2) : 0.f;
+    if (FROM_GLOBAL && j == 0) shift[row] = s;
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-      if (FROM_GLOBAL) v[r] = __ldcs(gsrc + row * N2 + j + r * T);
-      else v[r] = src[row * PITCH + pad(j + r * T)];
+      if (FROM_GLOBAL) {
+        v[r] = __ldcs(gsrc + row * N2 + j + r * T);
+        v[r] = make_float2(__fsub_rn(v[r].x, s), __fsub_rn(v[r].y, s));
+      } else {
+        v[r] = src[row * PITCH + pad(j + r * T)];
+      }
     }
     const int q = j / NS;
     const int k = j - q * NS;
@@ -360,6 +389,7 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_fixed_kernel(const SpecPa
   float2* buf_b = buf_a + size_t(p.rows_per_block) * PITCH;
   float2* tw2 = buf_b + size_t(p.rows_per_block) * PITCH;
   float2* twn = tw2 + N2;
+  __shared__ float shift[kSpMaxRows];  // per row of the block: the first stage's shift
 
   for (int i = threadIdx.x; i < N2; i += kSpThreads) tw2[i] = p.tw2[i];
   for (int i = threadIdx.x; i <= N2; i += kSpThreads) twn[i] = p.twn[i];
@@ -373,6 +403,7 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_fixed_kernel(const SpecPa
 
   constexpr int kPairIters = kSpMaxAcc / 2;
   float acc_lo[kPairIters], acc_hi[kPairIters];
+  float acc_dc = 0.f, acc_ny = 0.f;  // bins 0 and N2 of row threadIdx.x
 #pragma unroll
   for (int i = 0; i < kPairIters; ++i) { acc_lo[i] = 0.f; acc_hi[i] = 0.f; }
 
@@ -380,15 +411,15 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_fixed_kernel(const SpecPa
     const int64_t field = int64_t(ti) * p.nfield_out + slot;
     const float2* g =
         reinterpret_cast<const float2*>(p.x + (field * p.nrow + row0) * int64_t(2 * N2));
-    stage_ct<R0, 1, N2, true>(nullptr, buf_a, g, tw2, nrows);
+    stage_ct<R0, 1, N2, true>(nullptr, buf_a, g, tw2, nrows, shift);
     __syncthreads();
     const float2* z = buf_a;
     if (R1 > 1) {
-      stage_ct<R1, R0, N2, false>(buf_a, buf_b, g, tw2, nrows);
+      stage_ct<R1, R0, N2, false>(buf_a, buf_b, g, tw2, nrows, shift);
       __syncthreads();
       z = buf_b;
       if (R2 > 1) {
-        stage_ct<R2, R0 * R1, N2, false>(buf_b, buf_a, g, tw2, nrows);
+        stage_ct<R2, R0 * R1, N2, false>(buf_b, buf_a, g, tw2, nrows, shift);
         __syncthreads();
         z = buf_a;
       }
@@ -396,9 +427,9 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_fixed_kernel(const SpecPa
 #pragma unroll
     for (int it = 0; it < kPairIters; ++it) {
       const int idx = threadIdx.x + it * kSpThreads;
-      if (idx < total_pairs) {
-        const int row = idx / NPAIR;
-        const int k = idx - row * NPAIR;
+      const int row = idx / NPAIR;
+      const int k = idx - row * NPAIR;
+      if (idx < total_pairs && k != 0) {
         const float2 zk = z[row * PITCH + pad(k)];
         float2 zc = z[row * PITCH + pad(k == 0 ? 0 : N2 - k)];
         zc.y = -zc.y;
@@ -412,26 +443,41 @@ __global__ void __launch_bounds__(kSpThreads) spectrum_fixed_kernel(const SpecPa
         acc_hi[it] += (xb.x * xb.x + xb.y * xb.y) * 2.f * sc;
       }
     }
+    // bins 0 and N2 of row threadIdx.x: X_0 = Re Z_0 + Im Z_0 + N s (the shift
+    // back), X_N2 = Re Z_0 - Im Z_0 (the shift cancels)
+    if (threadIdx.x < nrows) {
+      const int row = threadIdx.x;
+      const float2 z0 = z[row * PITCH];
+      const float x0 = (z0.x + z0.y) + float(2 * N2) * shift[row], xn = z0.x - z0.y;
+      const float sc = p.scale[row0 + row];
+      acc_dc += x0 * x0 * sc;
+      acc_ny += xn * xn * 2.f * sc;
+    }
     __syncthreads();  // buffers are reused by the next time step
   }
 
 #pragma unroll
   for (int it = 0; it < kPairIters; ++it) {
     const int idx = threadIdx.x + it * kSpThreads;
-    if (idx < total_pairs) {
-      const int row = idx / NPAIR;
-      const int k = idx - row * NPAIR;
+    const int row = idx / NPAIR;
+    const int k = idx - row * NPAIR;
+    if (idx < total_pairs && k != 0) {
       float* o = p.out + ((slot * p.nrow + row0 + row) * int64_t(NK));
       o[k] = p.accumulate ? o[k] + acc_lo[it] : acc_lo[it];
       if (2 * k != N2) o[N2 - k] = p.accumulate ? o[N2 - k] + acc_hi[it] : acc_hi[it];
     }
+  }
+  if (threadIdx.x < nrows) {
+    float* o = p.out + ((slot * p.nrow + row0 + threadIdx.x) * int64_t(NK));
+    o[0] = p.accumulate ? o[0] + acc_dc : acc_dc;
+    o[N2] = p.accumulate ? o[N2] + acc_ny : acc_ny;
   }
 }
 
 template <int N2, int R0, int R1, int R2>
 static int launch_fixed(wb2_ctx* ctx, const SpecParams& p, size_t smem, unsigned grid) {
   auto kernel = spectrum_fixed_kernel<N2, R0, R1, R2>;
-  if (smem > 48 * 1024)
+  if (smem + kSpStaticSmem > 48 * 1024)
     WB2_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       static_cast<int>(smem)));
   kernel<<<grid, kSpThreads, smem, ctx->stream>>>(p);
@@ -479,15 +525,20 @@ static bool factorize(int n2, int* radix, int* nstage) {
 int spectrum_pfa_try(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t nrow, int32_t ncol,
                      const double* scale, float* out, int mode, int64_t nslot);
 
-// out[slot][k] = sum_row spec[slot][row][k]   (rows already carry their weights)
-__global__ void latsum_rows_kernel(const float* __restrict__ spec, float* __restrict__ out,
-                                   int64_t nslot, int nrow, int nk, int accumulate) {
+// out[slot][k] = sum_row spec[slot][row][k]   (rows already carry their weights;
+// rows of zero weight are skipped, so that a NaN or inf outside a latitude band
+// does not reach the band's sum as 0 * NaN)
+__global__ void latsum_rows_kernel(const float* __restrict__ spec,
+                                   const unsigned char* __restrict__ keep,
+                                   float* __restrict__ out, int64_t nslot, int nrow, int nk,
+                                   int accumulate) {
   const int64_t i = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
   if (i >= nslot * nk) return;
   const int64_t slot = i / nk;
   const int k = static_cast<int>(i - slot * nk);
   float s = 0.f;
-  for (int r = 0; r < nrow; ++r) s += spec[(slot * nrow + r) * int64_t(nk) + k];
+  for (int r = 0; r < nrow; ++r)
+    if (keep[r]) s += spec[(slot * nrow + r) * int64_t(nk) + k];
   out[i] = accumulate ? out[i] + s : s;
 }
 
@@ -516,11 +567,17 @@ int spectrum_latsum_impl(wb2_ctx* ctx, const float* x, int64_t nfield, int32_t n
   float* spec = static_cast<float*>(ctx->scratch);
   WB2_CUDA_TRY(cudaMemsetAsync(spec, 0, need, ctx->stream));
   WB2_TRY(wb2_zonal_spectrum(ctx, x, nfield, nrow, ncol, scale, spec, 1, nfield_out));
+  std::vector<unsigned char> keep(nrow);
+  for (int r = 0; r < nrow; ++r) keep[r] = scale[r] != 0.0;
+  Packer pk(ctx);
+  const size_t ok = pk.add(keep.data(), keep.size());
+  WB2_TRY(pk.commit());
   const int64_t n = nfield_out * nk;
   latsum_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, ctx->stream>>>(
-      spec, out, nfield_out, nrow, nk, accumulate);
+      spec, pk.dev<unsigned char>(ok), out, nfield_out, nrow, nk, accumulate);
   WB2_CUDA_TRY(cudaGetLastError());
   ctx->launches += 1;
+  WB2_TRY(pk.release());
   return WB2_OK;
 }
 
@@ -548,6 +605,8 @@ extern "C" int wb2_zonal_spectrum(wb2_ctx* ctx, const float* x, int64_t nfield, 
   WB2_REQUIRE(nfield_out > 0 && nfield % nfield_out == 0,
               "nfield (%lld) must be a multiple of nfield_out (%lld)",
               static_cast<long long>(nfield), static_cast<long long>(nfield_out));
+  // the Stockham kernels read each row as float2
+  WB2_REQUIRE((reinterpret_cast<uintptr_t>(x) & 7) == 0, "wb2_zonal_spectrum: x must be 8-byte aligned");
   if (ncol % 2 != 0) {
     set_error("wb2_zonal_spectrum: odd number of longitudes (%d) is not supported", ncol);
     return WB2_EUNSUPPORTED;
@@ -594,7 +653,7 @@ extern "C" int wb2_zonal_spectrum(wb2_ctx* ctx, const float* x, int64_t nfield, 
   p.row_pitch = p.n2 + (p.n2 >> 4) + 1;
   int rpb = static_cast<int>((46 * 1024) / (size_t(p.row_pitch) * sizeof(float2)));
   if (rpb < 1) rpb = 1;
-  if (rpb > 32) rpb = 32;
+  if (rpb > kSpMaxRows) rpb = kSpMaxRows;
   while (rpb > 1 && rpb * p.nk > kSpMaxAcc * kSpThreads) --rpb;
   WB2_REQUIRE(rpb * p.nk <= kSpMaxAcc * kSpThreads && rpb * p.nk < (1 << 20),
               "wb2_zonal_spectrum: %d longitudes exceed the supported row length", ncol);
@@ -619,7 +678,7 @@ extern "C" int wb2_zonal_spectrum(wb2_ctx* ctx, const float* x, int64_t nfield, 
   const int frc = try_fixed(ctx, p, smem, grid);
   if (frc < 0) return frc;
   if (frc == 0) {
-    if (smem > 48 * 1024)
+    if (smem + kSpStaticSmem > 48 * 1024)
       WB2_CUDA_TRY(cudaFuncSetAttribute(spectrum_kernel,
                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         static_cast<int>(smem)));

@@ -98,6 +98,17 @@ __device__ __forceinline__ u64 mul2(u64 a, u64 b) {
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
   return pk2(__fmaf_rn(lo2(a), lo2(b), lo2(c)), __fmaf_rn(hi2(a), hi2(b), hi2(c)));
 }
+// lane-wise c + a * s, leaving a lane alone whose s is 0: rows of zero weight
+// (outside a latitude band, or the padding row of an odd nrow) contribute
+// nothing, where 0 * inf or 0 * NaN would poison the sum
+__device__ __forceinline__ u64 fma2_w(u64 a, u64 s, u64 c) {
+  const float sl = lo2(s), sh = hi2(s);
+  return pk2(sl == 0.f ? lo2(c) : __fmaf_rn(lo2(a), sl, lo2(c)),
+             sh == 0.f ? hi2(c) : __fmaf_rn(hi2(a), sh, hi2(c)));
+}
+// the shift subtracted from a row before its transform: the row's first
+// element, or 0 when that is not finite (inf - inf would turn the row into NaN)
+__device__ __forceinline__ float row_shift(float x0) { return isfinite(x0) ? x0 : 0.f; }
 __device__ __forceinline__ C2 cadd(C2 a, C2 b) { return {add2(a.re, b.re), add2(a.im, b.im)}; }
 __device__ __forceinline__ C2 csub(C2 a, C2 b) { return {sub2(a.re, b.re), sub2(a.im, b.im)}; }
 // a * (wr + i wi), wr / wi compile-time constants (they become FFMA immediates)
@@ -280,7 +291,8 @@ struct Plan {
   static constexpr int kWorkBytes = G * N2 * 16;
   static constexpr int kTwnBytes = N2 * 16;
   static constexpr int kTaskBytes = ((NTC * 16 + 127) / 128) * 128;
-  static constexpr int kSmem = kStageBytes + kWorkBytes + kTwnBytes + kTaskBytes + 64;
+  // + the mbarrier (16 B) and the 2 G row shifts
+  static constexpr int kSmem = kStageBytes + kWorkBytes + kTwnBytes + kTaskBytes + 64 + 8 * G;
   // thread slots per row pair, padded to half-warps so that the 64-bit shared
   // accesses of a half-warp stay inside one row pair (conflict-free strides)
   static constexpr int PTB = (NTB + 15) / 16 * 16, PTC = (NTC + 15) / 16 * 16;
@@ -366,6 +378,7 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
                                                      P::kTwnBytes);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::kStageBytes + P::kWorkBytes +
                                                P::kTwnBytes + P::kTaskBytes);
+  float* const shift = reinterpret_cast<float*>(full + 2);  // [2 G] of the current item
   float* const tile = reinterpret_cast<float*>(work_re);  // flush tile [2 G][NK], aliases `work`
   const int tid = threadIdx.x;
 
@@ -389,13 +402,14 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
   // stage A (radix RA, staging -> work): half-warps share nC and span nB, so the
   // gathered LDS.64 hit 16 distinct bank pairs (SB is odd)
   const bool a_on = tid < G * P::NTA;
-  int a_e0 = 0, a_src = 0, a_dst = 0;
+  int a_e0 = 0, a_src = 0, a_dst = 0, a_g = 0;
   {
     const int g = tid / P::NTA, r = tid - g * P::NTA;
     const int nC = r / RB, nB = r - nC * RB;
     a_e0 = (P::SB * nB + P::SC * nC) % N2;
     a_src = 2 * g * N2;  // float2 index of row A of the pair; row B follows at + N2
     a_dst = g * N2 + nB * P::LB + nC;
+    a_g = g;
   }
   // stage B (radix RB, in place): consecutive threads, consecutive elements
   bool b_on;
@@ -406,7 +420,7 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
     b_off = g * N2 + r;
   }
   // stage C (radix RC on a butterfly and its mirror, then the real-input split)
-  int c_g = tid / P::PTC, c_off1 = 0, c_off2 = 0, c_k0 = 0, c_self = 0;
+  int c_g = tid / P::PTC, c_off1 = 0, c_off2 = 0, c_k0 = 0, c_self = 0;  // c_k0 == 0: owns bin 0
   const bool c_on = c_g < G && tid - c_g * P::PTC < P::NTC;
   if (c_on) {
     const int4 t = ctask[tid - c_g * P::PTC];
@@ -430,14 +444,22 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
     if (a_on) {
       const float2* ra = reinterpret_cast<const float2*>(staging) + a_src;
       const float2* rb = ra + N2;
+      // transform x - s (s = the row's first element): the DFT is shift-invariant
+      // except for bin 0, and the butterflies now round relative to the row's
+      // variation instead of its mean; stage C adds N s back to bin 0
+      const float sa = row_shift(ra[0].x), sb = row_shift(rb[0].x);
+      if (a_e0 == 0) {
+        shift[2 * a_g] = sa;
+        shift[2 * a_g + 1] = sb;
+      }
       C2 v[RA];
 #pragma unroll
       for (int nA = 0; nA < RA; ++nA) {
         int e = a_e0 + P::SA * nA;
         e = e >= N2 ? e - N2 : e;
         const float2 a = ra[e], b = rb[e];
-        v[nA].re = pk2v(a.x, b.x);
-        v[nA].im = pk2v(a.y, b.y);
+        v[nA].re = pk2v(__fsub_rn(a.x, sa), __fsub_rn(b.x, sb));
+        v[nA].im = pk2v(__fsub_rn(a.y, sa), __fsub_rn(b.y, sb));
       }
       dft<RA>(v);
 #pragma unroll
@@ -474,6 +496,11 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
       }
       dft<RC>(b1);
       dft<RC>(b2);
+      // 2 N s for the thread that owns bin 0 (the split computes 2 X_p), else 0
+      u64 dc = 0ull;
+      if (c_k0 == 0)
+        dc = pk2(__fmul_rn(float(2 * P::N), shift[2 * c_g]),
+                 __fmul_rn(float(2 * P::N), shift[2 * c_g + 1]));
       u64 scl = 0ull;
       if (MODE == 2) {
         const int row = 2 * (G * cur.gi + c_g);
@@ -490,13 +517,15 @@ __global__ void __launch_bounds__(P::NT, P::MINB) spectrum_pfa_kernel(const Para
         // W (-i D):  re = wr d_im + wi d_re,  im = wi d_im - wr d_re
         const u64 t1 = fma2(w.y, d_re, mul2(w.x, d_im));
         const u64 t2 = sub2(mul2(w.x, d_re), mul2(w.y, d_im));  // = -im
-        const u64 xa_re = add2(e_re, t1), xa_im = sub2(e_im, t2);
+        u64 xa_re = add2(e_re, t1);
+        const u64 xa_im = sub2(e_im, t2);
+        if (kC == 0) xa_re = add2(xa_re, dc);  // bin c_k0: the shift back into bin 0
         const u64 xb_re = sub2(e_re, t1), xb_im = add2(e_im, t2);
         if (MODE == 2) {
           const u64 pa = fma2(xa_im, xa_im, mul2(xa_re, xa_re));
           const u64 pb = fma2(xb_im, xb_im, mul2(xb_re, xb_re));
-          acc_a[kC] = fma2(pa, scl, acc_a[kC]);
-          acc_b[kC] = fma2(pb, scl, acc_b[kC]);
+          acc_a[kC] = fma2_w(pa, scl, acc_a[kC]);
+          acc_b[kC] = fma2_w(pb, scl, acc_b[kC]);
         } else {
           acc_a[kC] = fma2(xa_im, xa_im, fma2(xa_re, xa_re, acc_a[kC]));
           acc_b[kC] = fma2(xb_im, xb_im, fma2(xb_re, xb_re, acc_b[kC]));
