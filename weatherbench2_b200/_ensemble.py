@@ -17,7 +17,6 @@ from weatherbench2_b200 import metrics as m
 from weatherbench2_b200 import xarray_lite as xl
 
 REALIZATION = 'realization'
-LAT, LON = sp.LAT, sp.LON
 
 # indices into the K2 output (include/wb2b200.h, WB2_ENS_NSTAT)
 _SKILL, _SPREAD, _MSE, _VAR, _DEBIASED = 0, 1, 2, 3, 4
@@ -41,19 +40,13 @@ def _ens_stats(forecast: xl.Dataset, truth: xl.Dataset, ens_dim: str,
   """{var: (stats[..., R, 10], dims, coords, M)} from ONE pass over the
   ensemble (skill, spread, ens-mean SE, variance, debiased SE)."""
   ctx = m._context()  # pylint: disable=protected-access
-  names = m._common_vars(forecast, truth)  # pylint: disable=protected-access
   lat, lon = m._lat_lon(forecast)  # pylint: disable=protected-access
   out = {}
   groups: dict = {}
   prepared = {}
-  for name in names:
-    f_da, t_da = forecast[name], truth[name]
-    if LAT not in f_da.dims or LON not in f_da.dims:
-      continue
-    f_da, t_da = xl.align_inner(f_da, t_da)
-    # K2 computes in float32 (float64 inputs are rounded to float32 first)
-    x_op = sp.prepare_operand(f_da, None, np.float32)
-    t_op = sp.prepare_operand(t_da, x_op.layout, np.float32)
+  # K2 computes in float32 (float64 inputs are rounded to float32 first)
+  for name, f_da, t_da, x_op, t_op in m._paired_operands(  # pylint: disable=protected-access
+      forecast, truth, np.float32):
     prepared[name] = (x_op, t_op, f_da, t_da)
     groups.setdefault(m._group_key(x_op), []).append(name)  # pylint: disable=protected-access
   for _, members in groups.items():
@@ -69,17 +62,11 @@ def _ens_stats(forecast: xl.Dataset, truth: xl.Dataset, ens_dim: str,
 
 
 def _ens_request(forecast, truth, ens_dim, region, skipna) -> dict:
-  b = m._batch  # pylint: disable=protected-access
-  if b.active and m._region_index(region, b.regions) >= 0:  # pylint: disable=protected-access
-    key = ('ens', id(forecast), id(truth), ens_dim, bool(skipna))
-    if key not in b.cache:
-      b.cache[key] = (_ens_stats(forecast, truth, ens_dim, b.regions, skipna),
-                      forecast, truth)
-    res = b.cache[key][0]
-    ri = m._region_index(region, b.regions)  # pylint: disable=protected-access
-  else:
-    res = _ens_stats(forecast, truth, ens_dim, [region], skipna)
-    ri = 0
+  res, ri = m._region_request(  # pylint: disable=protected-access
+      ('ens', id(forecast), id(truth), ens_dim, bool(skipna)),
+      (forecast, truth),
+      lambda regions: _ens_stats(forecast, truth, ens_dim, regions, skipna),
+      region)
   return {k: (st[..., ri, :], dims, coords, mm)
           for k, (st, dims, coords, mm) in res.items()}
 
@@ -237,16 +224,10 @@ def _member_mean(ds: xl.Dataset, ens_dim: str, skipna: bool) -> xl.Dataset:
 def _energy_k3(forecast: xl.Dataset, truth: xl.Dataset, ens_dim: str, region):
   """(skill, spread) Datasets from ONE pass over the ensemble (K3)."""
   ctx = m._context()  # pylint: disable=protected-access
-  names = m._common_vars(forecast, truth)  # pylint: disable=protected-access
   lat, lon = m._lat_lon(forecast)  # pylint: disable=protected-access
   skill, spread = xl.Dataset(), xl.Dataset()
-  for name in names:
-    f_da, t_da = forecast[name], truth[name]
-    if LAT not in f_da.dims or LON not in f_da.dims:
-      continue
-    f_da, t_da = xl.align_inner(f_da, t_da)
-    x_op = sp.prepare_operand(f_da, None, np.float32)
-    t_op = sp.prepare_operand(t_da, x_op.layout, np.float32)
+  for name, f_da, t_da, x_op, t_op in m._paired_operands(  # pylint: disable=protected-access
+      forecast, truth, np.float32):
     (st,), (dims,), (mm,) = sp.run_energy_score(
         ctx, [x_op], [t_op], ens_dim, lat, lon, [region],
         m._global_cell_cache)  # pylint: disable=protected-access
@@ -342,13 +323,8 @@ def _ens_maps(forecast: xl.Dataset, truth: xl.Dataset, ens_dim: str,
   """{var: (maps[nsel, ...], dims, coords, M)} for the selected statistics."""
   ctx = m._context()  # pylint: disable=protected-access
   out = {}
-  for name in m._common_vars(forecast, truth):  # pylint: disable=protected-access
-    f_da, t_da = forecast[name], truth[name]
-    if LAT not in f_da.dims or LON not in f_da.dims:
-      continue
-    f_da, t_da = xl.align_inner(f_da, t_da)
-    x_op = sp.prepare_operand(f_da, None, np.float32)
-    t_op = sp.prepare_operand(t_da, x_op.layout, np.float32)
+  for name, f_da, t_da, x_op, t_op in m._paired_operands(  # pylint: disable=protected-access
+      forecast, truth, np.float32):
     maps, dims, mm = sp.run_ens_maps(ctx, x_op, t_op, ens_dim, stat_mask,
                                      reduce_dim, skipna)
     coords = m._map_coords(dims, f_da, t_da)  # pylint: disable=protected-access
@@ -360,14 +336,13 @@ def _ens_maps(forecast: xl.Dataset, truth: xl.Dataset, ens_dim: str,
 def _ens_map_request(forecast, truth, ens_dim, bit, reduce_dim, skipna):
   """One statistic's maps; inside `metrics.batch()` all six come from a single
   pass over the ensemble and are shared by the Spatial* metrics."""
-  b = m._batch  # pylint: disable=protected-access
-  if b.active:
-    key = ('ensmap', id(forecast), id(truth), ens_dim, reduce_dim,
-           bool(skipna))
-    if key not in b.cache:
-      b.cache[key] = (_ens_maps(forecast, truth, ens_dim, _ALL_MAPS,
-                                reduce_dim, skipna), forecast, truth)
-    res, sel = b.cache[key][0], _MAP_BITS.index(bit)
+  if m._batch.active:  # pylint: disable=protected-access
+    res = m._batch_cached(  # pylint: disable=protected-access
+        ('ensmap', id(forecast), id(truth), ens_dim, reduce_dim, bool(skipna)),
+        (forecast, truth),
+        lambda: _ens_maps(forecast, truth, ens_dim, _ALL_MAPS, reduce_dim,
+                          skipna))
+    sel = _MAP_BITS.index(bit)
   else:
     res, sel = _ens_maps(forecast, truth, ens_dim, bit, reduce_dim, skipna), 0
   out = xl.Dataset()

@@ -12,8 +12,6 @@ from weatherbench2_b200 import _spatial as sp
 from weatherbench2_b200 import metrics as m
 from weatherbench2_b200 import xarray_lite as xl
 
-LAT, LON = sp.LAT, sp.LON
-
 
 class RankHistogram(ens.EnsembleMetric):
   """Histogram of truth's rank with respect to the ensemble members.
@@ -61,16 +59,13 @@ class RankHistogram(ens.EnsembleMetric):
     if seed is None:
       seed = int(np.random.SeedSequence().entropy) & (2**64 - 1)
     ctx = m._context()  # pylint: disable=protected-access
+    names = m._common_vars(forecast, truth)  # pylint: disable=protected-access
     out = xl.Dataset()
-    for vi, name in enumerate(m._common_vars(forecast, truth)):  # pylint: disable=protected-access
-      f_da, t_da = forecast[name], truth[name]
-      if LAT not in f_da.dims or LON not in f_da.dims:
-        continue
-      f_da, t_da = xl.align_inner(f_da, t_da)
-      x_op = sp.prepare_operand(f_da, None, np.float32)
-      t_op = sp.prepare_operand(t_da, x_op.layout, np.float32)
-      hist, dims = _run(ctx, x_op, t_op, self.ensemble_dim, nbins, reduce_dim,
-                        self._break_ties_randomly, seed + vi)
+    for name, f_da, t_da, x_op, t_op in m._paired_operands(  # pylint: disable=protected-access
+        forecast, truth, np.float32):
+      hist, dims = sp.run_rank_histogram(
+          ctx, x_op, t_op, self.ensemble_dim, nbins, reduce_dim,
+          self._break_ties_randomly, seed + names.index(name))
       coords = m._map_coords(dims, f_da, t_da)  # pylint: disable=protected-access
       coords.pop(self.ensemble_dim, None)
       coords['bins'] = xl.Coord(('bins',), np.arange(nbins))
@@ -86,41 +81,6 @@ class RankHistogram(ens.EnsembleMetric):
     fc = xl.from_xarray(forecast)
     result = self._hist(forecast, truth, m._avg_dim(fc))  # pylint: disable=protected-access
     return result.assign_attrs(ensemble_size=fc.sizes[self.ensemble_dim])
-
-
-def _run(ctx, x_op, t_op, ens_dim, nbins, reduce_dim, random_ties, seed):
-  """Launches K10 for one variable.  Returns (hist[..., nrow, ncol, nbins],
-  dims without `bins`)."""
-  staged: list = []
-  try:
-    if ens_dim in t_op.outer_dims:
-      raise ValueError(f'truth must not have the {ens_dim!r} dimension')
-    was_dev = x_op.on_device
-    x_op = sp._to_device_operand(ctx, x_op, staged)  # pylint: disable=protected-access
-    t_op = sp._to_device_operand(ctx, t_op, staged)  # pylint: disable=protected-access
-    x_op, nmember, stride = sp.split_member_dim(x_op, ens_dim)
-    if (t_op.layout != x_op.layout or t_op.row_stride != x_op.row_stride or
-        t_op.nrow != x_op.nrow or t_op.ncol != x_op.ncol):
-      raise ValueError('forecast and truth must share layout and grid')
-    (off_x, off_t), out_dims, out_shape, ngroup = sp._grouped_tables(  # pylint: disable=protected-access
-        [x_op, t_op], reduce_dim)
-    nout = off_x.size // ngroup
-    shape = tuple(out_shape) + (x_op.nrow, x_op.ncol, nbins)
-    tensor, ptr = sp._alloc_maps(ctx, x_op if was_dev else t_op, shape,  # pylint: disable=protected-access
-                                 np.float32)
-    try:
-      ctx.rank_histogram(x_op.addr, t_op.addr, nmember, stride, nout, ngroup,
-                         off_x, off_t, x_op.nrow, x_op.ncol, x_op.row_stride,
-                         nbins, random_ties, seed, ptr)
-    except Exception:
-      if tensor is None:
-        ctx.free(ptr)
-      raise
-    hist = sp._fetch_maps(ctx, tensor, ptr, shape, np.float32)  # pylint: disable=protected-access
-    return hist, tuple(out_dims) + sp._map_dims(x_op)  # pylint: disable=protected-access
-  finally:
-    for p in staged:
-      ctx.free(p)
 
 
 def central_reliability(hist):

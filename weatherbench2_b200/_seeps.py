@@ -16,8 +16,6 @@ from weatherbench2_b200 import _spatial as sp
 from weatherbench2_b200 import metrics as m
 from weatherbench2_b200 import xarray_lite as xl
 
-LAT, LON = sp.LAT, sp.LON
-
 
 def _valid_time(da: xl.DataArray):
   """(dims, timestamps) of `da.valid_time` (metrics.py:446-448); data indexed
@@ -79,47 +77,10 @@ class SpatialSEEPS(m.Metric):
     f_op = sp.prepare_operand(f_da, None, np.float32)
     t_op = sp.prepare_operand(t_da, f_op.layout, np.float32)
     w_op = sp.prepare_operand(wet_da, f_op.layout, np.float32)
-    p1 = self.p1.transpose(*sp._map_dims(f_op))  # pylint: disable=protected-access
-    p1_np = np.ascontiguousarray(np.asarray(p1.values), dtype=np.float32)
-    if p1_np.shape != (f_op.nrow, f_op.ncol):
-      raise ValueError(f'dry fraction grid {p1_np.shape} does not match the '
-                       f'data grid {(f_op.nrow, f_op.ncol)}')
-    staged: list = []
-    try:
-      was_dev = f_op.on_device
-      f_op = sp._to_device_operand(ctx, f_op, staged)  # pylint: disable=protected-access
-      t_op = sp._to_device_operand(ctx, t_op, staged)  # pylint: disable=protected-access
-      w_op = sp._to_device_operand(ctx, w_op, staged)  # pylint: disable=protected-access
-      if (t_op.layout != f_op.layout or t_op.row_stride != f_op.row_stride or
-          t_op.nrow != f_op.nrow or t_op.ncol != f_op.ncol or
-          w_op.nrow != f_op.nrow or w_op.ncol != f_op.ncol):
-        raise ValueError('forecast, truth and climatology must share the grid')
-      wf_op = sp.gather_operand(w_op, _threshold_maps(wet_da, f_da))
-      wt_op = sp.gather_operand(w_op, _threshold_maps(wet_da, t_da))
-      (off_f, off_t, off_wf, off_wt), out_dims, out_shape, ngroup = (
-          sp._grouped_tables([f_op, t_op, wf_op, wt_op], reduce_dim))  # pylint: disable=protected-access
-      p1_dev = ctx.to_device(p1_np)
-      staged.append(p1_dev)
-      nout = off_f.size // ngroup
-      shape = tuple(out_shape) + (f_op.nrow, f_op.ncol)
-      tensor, ptr = sp._alloc_maps(ctx, f_op if was_dev else t_op, shape,  # pylint: disable=protected-access
-                                   np.float32)
-      try:
-        ctx.seeps_maps(f_op.addr, t_op.addr, w_op.addr, p1_dev, nout, ngroup,
-                       off_f, off_t, off_wf, off_wt, f_op.nrow, f_op.ncol,
-                       f_op.row_stride, w_op.row_stride,
-                       np.float32(self.dry_threshold_mm / 1000.0),
-                       np.float32(self.min_p1), np.float32(self.max_p1),
-                       skipna, ptr)
-      except Exception:
-        if tensor is None:
-          ctx.free(ptr)
-        raise
-      maps = sp._fetch_maps(ctx, tensor, ptr, shape, np.float32)  # pylint: disable=protected-access
-    finally:
-      for p in staged:
-        ctx.free(p)
-    dims = tuple(out_dims) + sp._map_dims(f_op)  # pylint: disable=protected-access
+    maps, dims = sp.run_seeps_maps(
+        ctx, f_op, t_op, w_op, _threshold_maps(wet_da, f_da),
+        _threshold_maps(wet_da, t_da), self.p1, self.dry_threshold_mm / 1000.0,
+        self.min_p1, self.max_p1, reduce_dim, skipna)
     out = xl.Dataset()
     out[name] = xl.DataArray(maps, dims, m._map_coords(dims, f_da, t_da), name)  # pylint: disable=protected-access
     return out, native

@@ -333,77 +333,7 @@ def build_weights(ctx: _lib.Context, latitude: np.ndarray,
   return out
 
 
-# ---- launches ----------------------------------------------------------------
-def _common_base(ops: Sequence[Operand]) -> int:
-  return min(op.addr for op in ops)
-
-
-def run_det_metrics(ctx: _lib.Context, f_ops: Sequence[Operand],
-                    t_ops: Sequence[Operand],
-                    c_ops: Optional[Sequence[Operand]], latitude, longitude,
-                    regions: Sequence, skipna: bool, cell_cache=None):
-  """Runs K1 for a list of variables that share dtype / layout / grid.
-
-  Returns (stats, dims, shapes): stats[v] has shape outer_shape[v] +
-  (len(regions), DET_NSTAT).
-  """
-  nvar = len(f_ops)
-  first = f_ops[0]
-  on_dev = first.on_device
-  dtype_code = _lib.F32 if first.dtype == np.float32 else _lib.F64
-  es = first.itemsize
-  all_ops = list(f_ops) + list(t_ops) + (list(c_ops) if c_ops else [])
-  for op in all_ops:
-    if (op.on_device != on_dev or op.dtype != first.dtype or
-        op.layout != first.layout or op.nrow != first.nrow or
-        op.ncol != first.ncol or op.row_stride != first.row_stride):
-      raise ValueError('operands of one launch must share device, dtype, '
-                       'layout, grid and row stride')
-  base = _common_base(all_ops)
-  dims_list, shape_list, tabs = [], [], [[], [], []]
-  for v in range(nvar):
-    trio = [f_ops[v], t_ops[v]] + ([c_ops[v]] if c_ops else [])
-    dims, shape = broadcast_dims(*trio)
-    dims_list.append(dims)
-    shape_list.append(shape)
-    for k, op in enumerate(trio):
-      rel = (op.addr - base)
-      assert rel % es == 0
-      tabs[k].append(offset_table(op, dims, shape) + rel // es)
-  off_f = np.ascontiguousarray(np.concatenate(tabs[0]))
-  off_t = np.ascontiguousarray(np.concatenate(tabs[1]))
-  off_c = np.ascontiguousarray(np.concatenate(tabs[2])) if c_ops else None
-  nfield = off_f.size
-  nreg = len(regions)
-  result = np.empty((nfield, nreg, _lib.DET_NSTAT), dtype=np.float64)
-  groups = build_weights(ctx, np.asarray(latitude), np.asarray(longitude),
-                         regions, first.layout, first.row_stride, cell_cache)
-  for ids, spec in groups:
-    R = len(ids)
-    if on_dev:
-      out_dev = ctx.malloc(nfield * R * _lib.DET_NSTAT * 8)
-      try:
-        ctx.det_metrics(base, base, base if c_ops else None, dtype_code, off_f,
-                        off_t, off_c, spec, skipna, out_dev)
-        part = ctx.from_device(out_dev, (nfield, R, _lib.DET_NSTAT),
-                               np.float64)
-      finally:
-        ctx.free(out_dev)
-    else:
-      part = np.empty((nfield, R, _lib.DET_NSTAT), dtype=np.float64)
-      ctx.det_metrics(base, base, base if c_ops else None, dtype_code, off_f,
-                      off_t, off_c, spec, skipna, part.ctypes.data, host=True)
-    result[:, ids, :] = part
-  stats, pos = [], 0
-  for v in range(nvar):
-    n = int(np.prod(shape_list[v])) if shape_list[v] else 1
-    stats.append(result[pos:pos + n].reshape(
-        shape_list[v] + (nreg, _lib.DET_NSTAT)))
-    pos += n
-  return stats, dims_list, shape_list
-
-
-# ---- K2: ensemble metrics ----------------------------------------------------
+# ---- ensemble members and gathered uploads ------------------------------------
 def split_member_dim(op: Operand, ens_dim: str):
   """Removes `ens_dim` from the outer dims of `op`; returns (op', M, stride)."""
   if ens_dim not in op.outer_dims:
@@ -491,97 +421,230 @@ def _upload_gathered(ctx: _lib.Context, op: Operand, staged: list) -> Operand:
   return out
 
 
-def _to_device_operand(ctx: _lib.Context, op: Operand, staged: list) -> Operand:
-  """Uploads a host operand to the device: the smallest contiguous span of its
-  backing array (same strides), or, for a gathered operand, only the slabs it
-  references."""
-  if op.on_device:
-    return op
-  if getattr(op, 'gather_terms', None) is not None:
-    return _upload_gathered(ctx, op, staged)
-  arr = op.data
-  base = arr
-  while isinstance(base, np.ndarray) and base.base is not None and isinstance(
-      base.base, np.ndarray):
-    base = base.base
-  # upload the smallest contiguous span that covers the view
-  lo = arr.ctypes.data
-  span = 1 + sum((n - 1) * abs(s) for n, s in zip(arr.shape, arr.strides)
-                 ) // arr.itemsize if arr.size else 1
-  flat = np.ctypeslib.as_array(
-      (np.ctypeslib.ctypes.c_char * (span * arr.itemsize)).from_address(lo))
-  dptr = ctx.to_device(flat)
-  staged.append(dptr)
-  out = dataclasses.replace(op, addr=dptr, on_device=True)
-  if hasattr(op, 'gather_terms'):
-    out.gather_terms = op.gather_terms
-  return out
+# ---- launch plumbing -----------------------------------------------------------
+class Staging:
+  """Device copies of host operands for one launch, freed when the `with`
+  block exits, also when the launch raises."""
+
+  def __init__(self, ctx: _lib.Context):
+    self.ctx = ctx
+    self.ptrs: list = []
+
+  def __enter__(self) -> 'Staging':
+    return self
+
+  def __exit__(self, *exc):
+    for p in self.ptrs:
+      self.ctx.free(p)
+
+  def array(self, arr: np.ndarray) -> int:
+    """Device copy of a host array."""
+    ptr = self.ctx.to_device(arr)
+    self.ptrs.append(ptr)
+    return ptr
+
+  def upload(self, op: Operand) -> Operand:
+    """`op` re-addressed on the device: the smallest contiguous span of its
+    backing array (same strides), or, for a gathered operand, only the slabs it
+    references.  Device operands are returned as they are."""
+    if op.on_device:
+      return op
+    if getattr(op, 'gather_terms', None) is not None:
+      return _upload_gathered(self.ctx, op, self.ptrs)
+    arr = op.data
+    lo = arr.ctypes.data
+    span = 1 + sum((n - 1) * abs(s) for n, s in zip(arr.shape, arr.strides)
+                   ) // arr.itemsize if arr.size else 1
+    flat = np.ctypeslib.as_array(
+        (np.ctypeslib.ctypes.c_char * (span * arr.itemsize)).from_address(lo))
+    out = dataclasses.replace(op, addr=self.array(flat), on_device=True)
+    if hasattr(op, 'gather_terms'):
+      out.gather_terms = op.gather_terms
+    return out
 
 
+_GRID = ('layout', 'nrow', 'ncol', 'row_stride')
+
+
+def _check_grid(ops: Sequence[Operand], fields: tuple = _GRID, dtype=None):
+  """Operands of one launch share one slab geometry: every operand agrees
+  with the first on `fields` and, when given, has `dtype`."""
+  first = ops[0]
+  for op in ops[1:]:
+    for f in fields:
+      if getattr(op, f) != getattr(first, f):
+        raise ValueError(f'operands of one launch must share {f}: '
+                         f'{getattr(first, f)} vs {getattr(op, f)}')
+  if dtype is not None:
+    for op in ops:
+      if op.dtype != dtype:
+        raise ValueError(f'this kernel takes {np.dtype(dtype)} operands, not '
+                         f'{op.dtype}')
+
+
+def _check_truth(t_op: Operand, ens_dim: str):
+  if ens_dim in t_op.outer_dims:
+    raise ValueError(f'truth must not have the {ens_dim!r} dimension')
+
+
+def addressing(ops: Sequence[Operand], dims: tuple, shape: tuple,
+                base: Optional[int] = None):
+  """(base, tables): the lowest address of `ops` (unless `base` is given) and
+  the element offsets of every operand's slabs over the (dims, shape) grid,
+  relative to it."""
+  if base is None:
+    base = min(op.addr for op in ops)
+  tabs = []
+  for op in ops:
+    rel = op.addr - base
+    assert rel % op.itemsize == 0
+    tabs.append(offset_table(op, dims, shape) + rel // op.itemsize)
+  return base, tabs
+
+
+def _reduce_last(dims: tuple, shape: tuple, reduce_dim: Optional[str]):
+  """The grid with `reduce_dim` (if present) moved last, for the map kernels
+  that average over it: returns (dims, shape, out_dims, out_shape, ngroup)."""
+  if reduce_dim is None or reduce_dim not in dims:
+    return dims, shape, dims, shape, 1
+  i = dims.index(reduce_dim)
+  out_dims, out_shape = dims[:i] + dims[i + 1:], shape[:i] + shape[i + 1:]
+  return (out_dims + (reduce_dim,), out_shape + (shape[i],), out_dims,
+          out_shape, shape[i])
+
+
+def _map_dims(op: Operand):
+  return (LAT, LON) if op.layout == 'lat_lon' else (LON, LAT)
+
+
+def run_region_groups(ctx: _lib.Context, groups, shape: tuple, axis: int,
+                      launch, host: bool = False) -> np.ndarray:
+  """Runs `launch(weights, out)` once per `build_weights` group and returns
+  the float64 result of `shape`, whose axis `axis` indexes the regions.  Each
+  launch writes the group's part (`shape` with that axis cut to the group)
+  into a device buffer, or, with `host`, straight into host memory."""
+  res = np.empty(shape, dtype=np.float64)
+  for ids, spec in groups:
+    part_shape = shape[:axis] + (len(ids),) + shape[axis + 1:]
+    if host:
+      part = np.empty(part_shape, dtype=np.float64)
+      launch(spec, part.ctypes.data)
+    else:
+      out = ctx.malloc(int(np.prod(part_shape)) * 8)
+      try:
+        launch(spec, out)
+        part = ctx.from_device(out, part_shape, np.float64)
+      finally:
+        ctx.free(out)
+    res[(slice(None),) * axis + (ids,)] = part
+  return res
+
+
+def _run_maps(ctx: _lib.Context, forecast: Operand, truth: Operand,
+              shape: tuple, dtype, launch):
+  """Runs `launch(out)` into new output maps of `shape`.  They are a torch
+  tensor left on the device when the forecast is a torch CUDA tensor (else
+  when the truth is), otherwise NumPy copied back from a raw allocation."""
+  src = forecast if xl._is_torch(forecast.data) else truth  # pylint: disable=protected-access
+  if xl._is_torch(src.data):  # pylint: disable=protected-access
+    import torch  # pylint: disable=import-outside-toplevel
+    maps = torch.empty(shape, dtype=getattr(torch, np.dtype(dtype).name),
+                       device=src.data.device)
+    launch(int(maps.data_ptr()))
+    return maps
+  out = ctx.malloc(max(int(np.prod(shape)) * np.dtype(dtype).itemsize, 16))
+  try:
+    launch(out)
+    return ctx.from_device(out, shape, dtype)
+  finally:
+    ctx.free(out)
+
+
+# ---- K1: deterministic metrics -------------------------------------------------
+def run_det_metrics(ctx: _lib.Context, f_ops: Sequence[Operand],
+                    t_ops: Sequence[Operand],
+                    c_ops: Optional[Sequence[Operand]], latitude, longitude,
+                    regions: Sequence, skipna: bool, cell_cache=None):
+  """Runs K1 for a list of variables that share dtype / layout / grid.
+
+  Returns (stats, dims, shapes): stats[v] has shape outer_shape[v] +
+  (len(regions), DET_NSTAT).
+  """
+  first = f_ops[0]
+  all_ops = list(f_ops) + list(t_ops) + (list(c_ops) if c_ops else [])
+  _check_grid(all_ops, _GRID + ('on_device', 'dtype'))
+  base = min(op.addr for op in all_ops)
+  dims_list, shape_list, tabs = [], [], [[], [], []]
+  for v in range(len(f_ops)):
+    trio = [f_ops[v], t_ops[v]] + ([c_ops[v]] if c_ops else [])
+    dims, shape = broadcast_dims(*trio)
+    dims_list.append(dims)
+    shape_list.append(shape)
+    for k, tab in enumerate(addressing(trio, dims, shape, base)[1]):
+      tabs[k].append(tab)
+  off_f, off_t, off_c = (np.ascontiguousarray(np.concatenate(t)) if t else None
+                         for t in tabs)
+  c = base if c_ops else None
+  code = _lib.F32 if first.dtype == np.float32 else _lib.F64
+  nreg = len(regions)
+  groups = build_weights(ctx, np.asarray(latitude), np.asarray(longitude),
+                         regions, first.layout, first.row_stride, cell_cache)
+  host = not first.on_device
+  result = run_region_groups(
+      ctx, groups, (off_f.size, nreg, _lib.DET_NSTAT), 1,
+      lambda w, out: ctx.det_metrics(base, base, c, code, off_f, off_t, off_c,
+                                     w, skipna, out, host=host), host)
+  stats, pos = [], 0
+  for shape in shape_list:
+    n = int(np.prod(shape)) if shape else 1
+    stats.append(result[pos:pos + n].reshape(shape + (nreg, _lib.DET_NSTAT)))
+    pos += n
+  return stats, dims_list, shape_list
+
+
+# ---- K2: ensemble metrics ----------------------------------------------------
 def run_ens_metrics(ctx: _lib.Context, x_ops: Sequence[Operand],
                     t_ops: Sequence[Operand], ens_dim: str, latitude,
                     longitude, regions: Sequence, skipna: bool,
                     cell_cache=None):
   """Runs K2 for variables sharing layout / grid.  Returns (stats, dims,
   shapes, M): stats[v] has shape outer_shape[v] + (len(regions), ENS_NSTAT)."""
-  staged: list = []
   # all-host float32 operands: stream member / truth slabs through the staging
   # buffers (wb2_ens_metrics_host; truth slabs go through the slab cache)
   host = all(not o.on_device and o.dtype == np.float32
              for o in list(x_ops) + list(t_ops))
-  try:
-    xs, ts, ms, strides = [], [], [], []
+  with Staging(ctx) as stage:
+    pairs = []
     for xo, to in zip(x_ops, t_ops):
-      if ens_dim in to.outer_dims:
-        raise ValueError(f'truth must not have the {ens_dim!r} dimension')
+      _check_truth(to, ens_dim)
       if not host:
-        xo = _to_device_operand(ctx, xo, staged)
-        to = _to_device_operand(ctx, to, staged)
-      xo, m, st = split_member_dim(xo, ens_dim)
-      xs.append(xo)
-      ts.append(to)
-      ms.append(m)
-      strides.append(st)
-    first = xs[0]
+        xo, to = stage.upload(xo), stage.upload(to)
+      pairs.append(split_member_dim(xo, ens_dim) + (to,))
+    first = pairs[0][0]
     nreg = len(regions)
     groups = build_weights(ctx, np.asarray(latitude), np.asarray(longitude),
                            regions, first.layout, first.row_stride, cell_cache)
-    stats, dims_list, shape_list = [], [], []
-    for xo, to, m, st in zip(xs, ts, ms, strides):
-      if (to.layout != xo.layout or to.row_stride != xo.row_stride or
-          to.nrow != xo.nrow or to.ncol != xo.ncol):
-        raise ValueError('forecast and truth must share layout and grid')
+    stats, dims_list, shape_list, ms = [], [], [], []
+    for xo, m, st, to in pairs:
+      _check_grid([xo, to])
       # xarray puts truth's dims first for abs(truth - forecast)
       # (metrics.py:824); we keep the forecast-first order used by every other
       # metric of this module and of the reference's `mean/var` based ones.
       dims, shape = broadcast_dims(xo, to)
-      base = min(xo.addr, to.addr)
-      off_x = offset_table(xo, dims, shape) + (xo.addr - base) // 4
-      off_t = offset_table(to, dims, shape) + (to.addr - base) // 4
-      nfield = off_x.size
-      res = np.empty((nfield, nreg, _lib.ENS_NSTAT), dtype=np.float64)
-      for ids, spec in groups:
-        if host:
-          part = np.empty((nfield, len(ids), _lib.ENS_NSTAT), np.float64)
-          ctx.ens_metrics_host(base, base, m, st, off_x, off_t, spec, skipna,
-                               part.ctypes.data)
-          res[:, ids, :] = part
-          continue
-        out_dev = ctx.malloc(nfield * len(ids) * _lib.ENS_NSTAT * 8)
-        try:
-          ctx.ens_metrics(base, base, _lib.F32, m, st, off_x, off_t, spec,
-                          skipna, out_dev)
-          res[:, ids, :] = ctx.from_device(
-              out_dev, (nfield, len(ids), _lib.ENS_NSTAT), np.float64)
-        finally:
-          ctx.free(out_dev)
+      base, (off_x, off_t) = addressing([xo, to], dims, shape)
+      if host:
+        launch = lambda w, out: ctx.ens_metrics_host(  # pylint: disable=cell-var-from-loop
+            base, base, m, st, off_x, off_t, w, skipna, out)
+      else:
+        launch = lambda w, out: ctx.ens_metrics(  # pylint: disable=cell-var-from-loop
+            base, base, _lib.F32, m, st, off_x, off_t, w, skipna, out)
+      res = run_region_groups(ctx, groups, (off_x.size, nreg, _lib.ENS_NSTAT),
+                              1, launch, host)
       stats.append(res.reshape(shape + (nreg, _lib.ENS_NSTAT)))
       dims_list.append(dims)
       shape_list.append(shape)
-    return stats, dims_list, shape_list, ms
-  finally:
-    for p in staged:
-      ctx.free(p)
+      ms.append(m)
+  return stats, dims_list, shape_list, ms
 
 
 # ---- K3: energy score --------------------------------------------------------
@@ -593,122 +656,46 @@ def run_energy_score(ctx: _lib.Context, x_ops: Sequence[Operand],
                      longitude, regions: Sequence, cell_cache=None):
   """Runs K3.  Returns (stats, dims, M): stats[v] has shape
   outer_shape[v] + (len(regions), 4, M) -- see wb2_energy_score."""
-  staged: list = []
-  try:
-    first = None
-    stats, dims_list, ms = [], [], []
+  groups = None
+  stats, dims_list, ms = [], [], []
+  with Staging(ctx) as stage:
     for xo, to in zip(x_ops, t_ops):
-      xo = _to_device_operand(ctx, xo, staged)
-      to = _to_device_operand(ctx, to, staged)
+      xo, to = stage.upload(xo), stage.upload(to)
       xo, m, st = split_member_dim(xo, ens_dim)
-      if first is None:
-        first = xo
+      if groups is None:
         groups = build_weights(ctx, np.asarray(latitude),
                                np.asarray(longitude), regions, xo.layout,
                                xo.row_stride, cell_cache, ENERGY_MAX_REGIONS)
       dims, shape = broadcast_dims(xo, to)
-      base = min(xo.addr, to.addr)
-      off_x = offset_table(xo, dims, shape) + (xo.addr - base) // 4
-      off_t = offset_table(to, dims, shape) + (to.addr - base) // 4
-      nfield = off_x.size
-      res = np.empty((nfield, len(regions), 4, m), dtype=np.float64)
-      for ids, spec in groups:
-        out_dev = ctx.malloc(nfield * len(ids) * 4 * m * 8)
-        try:
-          ctx.energy_score(base, base, _lib.F32, m, st, off_x, off_t, spec,
-                           out_dev)
-          res[:, ids] = ctx.from_device(out_dev, (nfield, len(ids), 4, m),
-                                        np.float64)
-        finally:
-          ctx.free(out_dev)
+      base, (off_x, off_t) = addressing([xo, to], dims, shape)
+      res = run_region_groups(
+          ctx, groups, (off_x.size, len(regions), 4, m), 1,
+          lambda w, out: ctx.energy_score(  # pylint: disable=cell-var-from-loop
+              base, base, _lib.F32, m, st, off_x, off_t, w, out))
       stats.append(res.reshape(shape + (len(regions), 4, m)))
       dims_list.append(dims)
       ms.append(m)
-    return stats, dims_list, ms
-  finally:
-    for p in staged:
-      ctx.free(p)
+  return stats, dims_list, ms
 
 
 # ---- K6: map-output metrics (time mean fused in) -------------------------------
-def _grouped_tables(ops: Sequence[Operand], reduce_dim: Optional[str]):
-  """Offset tables of `ops` over their broadcast outer grid with `reduce_dim`
-  (if present) moved last: returns (tables, out_dims, out_shape, ngroup)."""
-  dims, shape = broadcast_dims(*ops)
-  if reduce_dim is not None and reduce_dim in dims:
-    i = dims.index(reduce_dim)
-    ngroup = shape[i]
-    out_dims = dims[:i] + dims[i + 1:]
-    out_shape = shape[:i] + shape[i + 1:]
-    dims, shape = out_dims + (reduce_dim,), out_shape + (ngroup,)
-  else:
-    ngroup, out_dims, out_shape = 1, dims, shape
-  return ([offset_table(op, dims, shape) for op in ops], out_dims, out_shape,
-          ngroup)
-
-
-def _map_dims(op: Operand):
-  return (LAT, LON) if op.layout == 'lat_lon' else (LON, LAT)
-
-
-def _alloc_maps(ctx: _lib.Context, like: Operand, shape: tuple, dtype):
-  """Device buffer for the output maps: a torch tensor when the inputs are
-  torch CUDA tensors (the result stays on the device), else a raw allocation
-  that `_fetch_maps` copies back."""
-  if xl._is_torch(like.data):  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    out = torch.empty(shape, dtype=getattr(torch, np.dtype(dtype).name),
-                      device=like.data.device)
-    return out, int(out.data_ptr())
-  nbytes = int(np.prod(shape)) * np.dtype(dtype).itemsize
-  return None, ctx.malloc(max(nbytes, 16))
-
-
-def _fetch_maps(ctx: _lib.Context, tensor, ptr: int, shape: tuple, dtype):
-  if tensor is not None:
-    return tensor
-  try:
-    return ctx.from_device(ptr, shape, dtype)
-  finally:
-    ctx.free(ptr)
-
-
 def run_det_maps(ctx: _lib.Context, f_op: Operand, t_op: Operand, stat: int,
                  reduce_dim: Optional[str], skipna: bool):
   """Runs K6 for one variable: maps of stat(f, t) averaged over `reduce_dim`
   (None: no averaging).  Returns (maps, dims)."""
-  staged: list = []
-  try:
-    was_dev = f_op.on_device
-    f_op = _to_device_operand(ctx, f_op, staged)
-    t_op = _to_device_operand(ctx, t_op, staged)
-    if (t_op.layout != f_op.layout or t_op.row_stride != f_op.row_stride or
-        t_op.nrow != f_op.nrow or t_op.ncol != f_op.ncol or
-        t_op.dtype != f_op.dtype):
-      raise ValueError('forecast and truth must share dtype, layout and grid')
-    (off_f, off_t), out_dims, out_shape, ngroup = _grouped_tables(
-        [f_op, t_op], reduce_dim)
-    es = f_op.itemsize
-    base = min(f_op.addr, t_op.addr)
-    off_f = off_f + (f_op.addr - base) // es
-    off_t = off_t + (t_op.addr - base) // es
-    nout = off_f.size // ngroup
-    shape = tuple(out_shape) + (f_op.nrow, f_op.ncol)
-    tensor, ptr = _alloc_maps(ctx, f_op if was_dev else t_op, shape,
-                              f_op.dtype)
+  with Staging(ctx) as stage:
+    f_op, t_op = stage.upload(f_op), stage.upload(t_op)
+    _check_grid([f_op, t_op], _GRID + ('dtype',))
+    dims, shape, out_dims, out_shape, ngroup = _reduce_last(
+        *broadcast_dims(f_op, t_op), reduce_dim)
+    base, (off_f, off_t) = addressing([f_op, t_op], dims, shape)
     code = _lib.F32 if f_op.dtype == np.float32 else _lib.F64
-    try:
-      ctx.det_maps(base, base, code, stat, nout, ngroup, off_f, off_t,
-                   f_op.nrow, f_op.ncol, f_op.row_stride, skipna, ptr)
-    except Exception:
-      if tensor is None:
-        ctx.free(ptr)
-      raise
-    maps = _fetch_maps(ctx, tensor, ptr, shape, f_op.dtype)
-    return maps, tuple(out_dims) + _map_dims(f_op)
-  finally:
-    for p in staged:
-      ctx.free(p)
+    maps = _run_maps(
+        ctx, f_op, t_op, out_shape + (f_op.nrow, f_op.ncol), f_op.dtype,
+        lambda out: ctx.det_maps(base, base, code, stat, off_f.size // ngroup,
+                                 ngroup, off_f, off_t, f_op.nrow, f_op.ncol,
+                                 f_op.row_stride, skipna, out))
+  return maps, out_dims + _map_dims(f_op)
 
 
 def run_ens_maps(ctx: _lib.Context, x_op: Operand, t_op: Operand,
@@ -717,90 +704,56 @@ def run_ens_maps(ctx: _lib.Context, x_op: Operand, t_op: Operand,
   """Runs K6e for one variable.  Returns (maps[nsel, ...], dims, M): the
   selected point-wise ensemble statistics (increasing bit order of
   `stat_mask`) averaged over `reduce_dim`."""
-  staged: list = []
-  try:
-    if ens_dim in t_op.outer_dims:
-      raise ValueError(f'truth must not have the {ens_dim!r} dimension')
-    was_dev = x_op.on_device
-    x_op = _to_device_operand(ctx, x_op, staged)
-    t_op = _to_device_operand(ctx, t_op, staged)
+  _check_truth(t_op, ens_dim)
+  with Staging(ctx) as stage:
+    x_op, t_op = stage.upload(x_op), stage.upload(t_op)
     x_op, m, st = split_member_dim(x_op, ens_dim)
-    if (t_op.layout != x_op.layout or t_op.row_stride != x_op.row_stride or
-        t_op.nrow != x_op.nrow or t_op.ncol != x_op.ncol):
-      raise ValueError('forecast and truth must share layout and grid')
-    if x_op.dtype != np.float32 or t_op.dtype != np.float32:
-      raise ValueError('ensemble kernels take float32 operands')
-    (off_x, off_t), out_dims, out_shape, ngroup = _grouped_tables(
-        [x_op, t_op], reduce_dim)
-    base = min(x_op.addr, t_op.addr)
-    off_x = off_x + (x_op.addr - base) // 4
-    off_t = off_t + (t_op.addr - base) // 4
-    nout = off_x.size // ngroup
+    _check_grid([x_op, t_op], dtype=np.float32)
+    dims, shape, out_dims, out_shape, ngroup = _reduce_last(
+        *broadcast_dims(x_op, t_op), reduce_dim)
+    base, (off_x, off_t) = addressing([x_op, t_op], dims, shape)
     nsel = bin(stat_mask).count('1')
-    shape = (nsel,) + tuple(out_shape) + (x_op.nrow, x_op.ncol)
-    tensor, ptr = _alloc_maps(ctx, x_op if was_dev else t_op, shape,
-                              np.float32)
-    try:
-      ctx.ens_maps(base, base, _lib.F32, m, st, nout, ngroup, off_x, off_t,
-                   x_op.nrow, x_op.ncol, x_op.row_stride, stat_mask, skipna,
-                   ptr)
-    except Exception:
-      if tensor is None:
-        ctx.free(ptr)
-      raise
-    maps = _fetch_maps(ctx, tensor, ptr, shape, np.float32)
-    return maps, tuple(out_dims) + _map_dims(x_op), m
-  finally:
-    for p in staged:
-      ctx.free(p)
+    maps = _run_maps(
+        ctx, x_op, t_op, (nsel,) + out_shape + (x_op.nrow, x_op.ncol),
+        np.float32,
+        lambda out: ctx.ens_maps(base, base, _lib.F32, m, st,
+                                 off_x.size // ngroup, ngroup, off_x, off_t,
+                                 x_op.nrow, x_op.ncol, x_op.row_stride,
+                                 stat_mask, skipna, out))
+  return maps, out_dims + _map_dims(x_op), m
 
 
 # ---- K7: threshold / Gaussian metrics -----------------------------------------
 THR_NOUT = 8
 
 
-def _threshold_tables(spec, dims, shape, base, staged, ctx):
-  """Device addressing of a threshold spec over the broadcast outer grid.
-  spec: ('field', [op per threshold]) or ('gaussian', mean_op, std_op, [z]).
-  Returns (nq, ops_on_device, builder) where builder(base) -> kernel args."""
-  if spec[0] == 'field':
-    seen: dict = {}  # thresholds that share a climatology array share its upload
+def _threshold_operands(spec, stage: Staging):
+  """Stages the threshold operands of `spec`: ('field', [op per threshold]),
+  ('gaussian', mean_op, std_op, [z]) or None (no thresholds).  Returns (ops,
+  args): args(base, tables) -> the kernel's (nq, thr_a, off_a, thr_b, off_b,
+  z) from the offset tables of `ops` relative to `base`."""
+  if spec is None:
+    return [], lambda base, tabs: (0, None, None, None, None, None)
+  if spec[0] == 'gaussian':
+    ops = [stage.upload(spec[1]), stage.upload(spec[2])]
+    z = np.asarray(spec[3], dtype=np.float64)
+    return ops, lambda base, tabs: (z.size, base, tabs[0], base, tabs[1], z)
+  seen: dict = {}  # thresholds that share a climatology array share its upload
 
-    def stage(op):
-      if op.on_device:
-        return op
-      if getattr(op, 'gather_terms', None) is not None:
-        # a gathered threshold field (day-of-year / quantile lookup): only the
-        # slabs it references are uploaded, re-addressed by the returned operand
-        return _to_device_operand(ctx, op, staged)
-      key = id(op.data)
-      if key not in seen:
-        seen[key] = _to_device_operand(ctx, op, staged).addr
-      return dataclasses.replace(op, addr=seen[key], on_device=True)
+  def one(op):
+    if op.on_device or getattr(op, 'gather_terms', None) is not None:
+      # a gathered threshold field (day-of-year / quantile lookup): only the
+      # slabs it references are uploaded, re-addressed by the returned operand
+      return stage.upload(op)
+    key = id(op.data)
+    if key not in seen:
+      seen[key] = stage.upload(op).addr
+    return dataclasses.replace(op, addr=seen[key], on_device=True)
 
-    ops = [stage(op) for op in spec[1]]
-    return len(ops), ops, lambda b: (
-        b, np.ascontiguousarray(np.concatenate([
-            offset_table(op, dims, shape) + (op.addr - b) // 4
-            for op in ops])), None, None, None)
-  m_op = _to_device_operand(ctx, spec[1], staged)
-  s_op = _to_device_operand(ctx, spec[2], staged)
-  z = np.asarray(spec[3], dtype=np.float64)
-  return z.size, [m_op, s_op], lambda b: (
-      b, offset_table(m_op, dims, shape) + (m_op.addr - b) // 4, b,
-      offset_table(s_op, dims, shape) + (s_op.addr - b) // 4, z)
-
-
-def _check_same_grid(first: Operand, others: Sequence[Operand]):
-  for op in others:
-    if (op.layout != first.layout or op.row_stride != first.row_stride or
-        op.nrow != first.nrow or op.ncol != first.ncol):
-      raise ValueError('operands must share layout, grid and row stride '
-                       f'({op.layout}, {op.nrow}x{op.ncol}, {op.row_stride}) vs '
-                       f'({first.layout}, {first.nrow}x{first.ncol}, '
-                       f'{first.row_stride})')
-    if op.dtype != np.float32:
-      raise ValueError('threshold / Gaussian kernels take float32 operands')
+  ops = [one(op) for op in spec[1]]
+  return ops, lambda base, tabs: (
+      len(ops), base, np.ascontiguousarray(np.concatenate(tabs)), None, None,
+      None)
 
 
 def run_ens_threshold_metrics(ctx: _lib.Context, x_op: Operand, t_op: Operand,
@@ -809,39 +762,23 @@ def run_ens_threshold_metrics(ctx: _lib.Context, x_op: Operand, t_op: Operand,
                               cell_cache=None):
   """Runs K7 (ensemble entry) for one variable.  Returns (stats, dims, M):
   stats has shape outer_shape + (nq, len(regions), 8)."""
-  staged: list = []
-  try:
-    if ens_dim in t_op.outer_dims:
-      raise ValueError(f'truth must not have the {ens_dim!r} dimension')
-    x_op = _to_device_operand(ctx, x_op, staged)
-    t_op = _to_device_operand(ctx, t_op, staged)
+  _check_truth(t_op, ens_dim)
+  with Staging(ctx) as stage:
+    x_op, t_op = stage.upload(x_op), stage.upload(t_op)
     x_op, m, st = split_member_dim(x_op, ens_dim)
     dims, shape = broadcast_dims(x_op, t_op)
-    nq, thr_ops, build = _threshold_tables(spec, dims, shape, 0, staged, ctx)
-    _check_same_grid(x_op, [t_op] + thr_ops)
-    base = min(op.addr for op in [x_op, t_op] + thr_ops)
-    off_x = offset_table(x_op, dims, shape) + (x_op.addr - base) // 4
-    off_t = offset_table(t_op, dims, shape) + (t_op.addr - base) // 4
-    thr_a, off_a, thr_b, off_b, z = build(base)
-    nfield = off_x.size
+    thr_ops, thr_args = _threshold_operands(spec, stage)
+    _check_grid([x_op, t_op] + thr_ops, dtype=np.float32)
+    base, tabs = addressing([x_op, t_op] + thr_ops, dims, shape)
+    nq, *thr = thr_args(base, tabs[2:])
     nreg = len(regions)
     groups = build_weights(ctx, np.asarray(latitude), np.asarray(longitude),
                            regions, x_op.layout, x_op.row_stride, cell_cache)
-    res = np.empty((nfield, nq, nreg, THR_NOUT), dtype=np.float64)
-    for ids, wspec in groups:
-      out_dev = ctx.malloc(nfield * nq * len(ids) * THR_NOUT * 8)
-      try:
-        ctx.ens_threshold_metrics(base, base, m, st, off_x, off_t, nq, thr_a,
-                                  off_a, thr_b, off_b, z, wspec, skipna,
-                                  out_dev)
-        res[:, :, ids, :] = ctx.from_device(
-            out_dev, (nfield, nq, len(ids), THR_NOUT), np.float64)
-      finally:
-        ctx.free(out_dev)
-    return res.reshape(shape + (nq, nreg, THR_NOUT)), dims, m
-  finally:
-    for p in staged:
-      ctx.free(p)
+    res = run_region_groups(
+        ctx, groups, (tabs[0].size, nq, nreg, THR_NOUT), 2,
+        lambda w, out: ctx.ens_threshold_metrics(
+            base, base, m, st, tabs[0], tabs[1], nq, *thr, w, skipna, out))
+  return res.reshape(shape + (nq, nreg, THR_NOUT)), dims, m
 
 
 def run_gaussian_metrics(ctx: _lib.Context, m_op: Operand, s_op: Operand,
@@ -849,41 +786,23 @@ def run_gaussian_metrics(ctx: _lib.Context, m_op: Operand, s_op: Operand,
                          regions: Sequence, skipna: bool, cell_cache=None):
   """Runs K7 (Gaussian entry) for one variable; spec None -> CRPS / variance.
   Returns (stats, dims): stats has shape outer_shape + (max(nq, 1), R, 8)."""
-  staged: list = []
-  try:
-    m_op = _to_device_operand(ctx, m_op, staged)
-    s_op = _to_device_operand(ctx, s_op, staged)
-    t_op = _to_device_operand(ctx, t_op, staged)
-    dims, shape = broadcast_dims(m_op, s_op, t_op)
-    if spec is not None:
-      nq, thr_ops, build = _threshold_tables(spec, dims, shape, 0, staged, ctx)
-    else:
-      nq, thr_ops, build = 0, [], lambda b: (None, None, None, None, None)
-    _check_same_grid(m_op, [s_op, t_op] + thr_ops)
-    base = min(op.addr for op in [m_op, s_op, t_op] + thr_ops)
-    off_m = offset_table(m_op, dims, shape) + (m_op.addr - base) // 4
-    off_s = offset_table(s_op, dims, shape) + (s_op.addr - base) // 4
-    off_t = offset_table(t_op, dims, shape) + (t_op.addr - base) // 4
-    thr_a, off_a, thr_b, off_b, z = build(base)
-    nfield = off_m.size
-    nreg = len(regions)
+  with Staging(ctx) as stage:
+    ops = [stage.upload(op) for op in (m_op, s_op, t_op)]
+    dims, shape = broadcast_dims(*ops)
+    thr_ops, thr_args = _threshold_operands(spec, stage)
+    _check_grid(ops + thr_ops, dtype=np.float32)
+    base, tabs = addressing(ops + thr_ops, dims, shape)
+    nq, *thr = thr_args(base, tabs[3:])
     nq_out = max(nq, 1)
+    nreg = len(regions)
     groups = build_weights(ctx, np.asarray(latitude), np.asarray(longitude),
-                           regions, m_op.layout, m_op.row_stride, cell_cache)
-    res = np.empty((nfield, nq_out, nreg, THR_NOUT), dtype=np.float64)
-    for ids, wspec in groups:
-      out_dev = ctx.malloc(nfield * nq_out * len(ids) * THR_NOUT * 8)
-      try:
-        ctx.gaussian_metrics(base, base, base, off_m, off_s, off_t, nq, thr_a,
-                             off_a, thr_b, off_b, z, wspec, skipna, out_dev)
-        res[:, :, ids, :] = ctx.from_device(
-            out_dev, (nfield, nq_out, len(ids), THR_NOUT), np.float64)
-      finally:
-        ctx.free(out_dev)
-    return res.reshape(shape + (nq_out, nreg, THR_NOUT)), dims
-  finally:
-    for p in staged:
-      ctx.free(p)
+                           regions, ops[0].layout, ops[0].row_stride,
+                           cell_cache)
+    res = run_region_groups(
+        ctx, groups, (tabs[0].size, nq_out, nreg, THR_NOUT), 2,
+        lambda w, out: ctx.gaussian_metrics(base, base, base, *tabs[:3], nq,
+                                            *thr, w, skipna, out))
+  return res.reshape(shape + (nq_out, nreg, THR_NOUT)), dims
 
 
 def run_ens_threshold_maps(ctx: _lib.Context, x_op: Operand, t_op: Operand,
@@ -891,43 +810,79 @@ def run_ens_threshold_maps(ctx: _lib.Context, x_op: Operand, t_op: Operand,
                            reduce_dim: Optional[str], skipna: bool):
   """Runs the map-output form of K7 for one variable.  Returns (maps, dims,
   M): maps[nq, ...outer (without reduce_dim)..., nrow, ncol] float32."""
-  staged: list = []
-  try:
-    if ens_dim in t_op.outer_dims:
-      raise ValueError(f'truth must not have the {ens_dim!r} dimension')
-    was_dev = x_op.on_device
-    x_op = _to_device_operand(ctx, x_op, staged)
-    t_op = _to_device_operand(ctx, t_op, staged)
+  _check_truth(t_op, ens_dim)
+  with Staging(ctx) as stage:
+    x_op, t_op = stage.upload(x_op), stage.upload(t_op)
     x_op, m, st = split_member_dim(x_op, ens_dim)
-    dims, shape = broadcast_dims(x_op, t_op)
-    if reduce_dim is not None and reduce_dim in dims:
-      i = dims.index(reduce_dim)
-      ngroup = shape[i]
-      out_dims = dims[:i] + dims[i + 1:]
-      out_shape = shape[:i] + shape[i + 1:]
-      dims, shape = out_dims + (reduce_dim,), out_shape + (ngroup,)
-    else:
-      ngroup, out_dims, out_shape = 1, dims, shape
-    nq, thr_ops, build = _threshold_tables(spec, dims, shape, 0, staged, ctx)
-    _check_same_grid(x_op, [t_op] + thr_ops)
-    base = min(op.addr for op in [x_op, t_op] + thr_ops)
-    off_x = offset_table(x_op, dims, shape) + (x_op.addr - base) // 4
-    off_t = offset_table(t_op, dims, shape) + (t_op.addr - base) // 4
-    thr_a, off_a, thr_b, off_b, z = build(base)
-    nout = off_x.size // ngroup
-    out_full = (nq,) + tuple(out_shape) + (x_op.nrow, x_op.ncol)
-    tensor, ptr = _alloc_maps(ctx, x_op if was_dev else t_op, out_full,
-                              np.float32)
-    try:
-      ctx.ens_threshold_maps(base, base, m, st, nout, ngroup, off_x, off_t, nq,
-                             thr_a, off_a, thr_b, off_b, z, x_op.nrow,
-                             x_op.ncol, x_op.row_stride, stat, skipna, ptr)
-    except Exception:
-      if tensor is None:
-        ctx.free(ptr)
-      raise
-    maps = _fetch_maps(ctx, tensor, ptr, out_full, np.float32)
-    return maps, tuple(out_dims) + _map_dims(x_op), m
-  finally:
-    for p in staged:
-      ctx.free(p)
+    dims, shape, out_dims, out_shape, ngroup = _reduce_last(
+        *broadcast_dims(x_op, t_op), reduce_dim)
+    thr_ops, thr_args = _threshold_operands(spec, stage)
+    _check_grid([x_op, t_op] + thr_ops, dtype=np.float32)
+    base, tabs = addressing([x_op, t_op] + thr_ops, dims, shape)
+    nq, *thr = thr_args(base, tabs[2:])
+    maps = _run_maps(
+        ctx, x_op, t_op, (nq,) + out_shape + (x_op.nrow, x_op.ncol),
+        np.float32,
+        lambda out: ctx.ens_threshold_maps(
+            base, base, m, st, tabs[0].size // ngroup, ngroup, tabs[0],
+            tabs[1], nq, *thr, x_op.nrow, x_op.ncol, x_op.row_stride, stat,
+            skipna, out))
+  return maps, out_dims + _map_dims(x_op), m
+
+
+# ---- K9: SEEPS maps, K10: rank histogram ------------------------------------------
+def run_seeps_maps(ctx: _lib.Context, f_op: Operand, t_op: Operand,
+                   wet_op: Operand, f_lookup: dict, t_lookup: dict, p1,
+                   dry_threshold: float, min_p1: float, max_p1: float,
+                   reduce_dim: Optional[str], skipna: bool):
+  """Runs K9 for one variable: SEEPS maps of (f, t) averaged over
+  `reduce_dim`.  The wet thresholds `wet_op` are looked up at the forecast's
+  and the truth's valid times through the `gather_operand` index maps
+  `f_lookup` / `t_lookup`; `p1` is the (latitude, longitude) DataArray of the
+  average dry fraction.  Returns (maps, dims)."""
+  p1 = np.ascontiguousarray(np.asarray(p1.transpose(*_map_dims(f_op)).values),
+                            dtype=np.float32)
+  if p1.shape != (f_op.nrow, f_op.ncol):
+    raise ValueError(f'dry fraction grid {p1.shape} does not match the '
+                     f'data grid {(f_op.nrow, f_op.ncol)}')
+  with Staging(ctx) as stage:
+    f_op, t_op, wet_op = (stage.upload(op) for op in (f_op, t_op, wet_op))
+    _check_grid([f_op, t_op])
+    # the threshold climatology keeps its own row stride
+    _check_grid([f_op, wet_op], ('nrow', 'ncol'))
+    ops = [f_op, t_op, gather_operand(wet_op, f_lookup),
+           gather_operand(wet_op, t_lookup)]
+    dims, shape, out_dims, out_shape, ngroup = _reduce_last(
+        *broadcast_dims(*ops), reduce_dim)
+    tabs = [offset_table(op, dims, shape) for op in ops]
+    p1_dev = stage.array(p1)
+    maps = _run_maps(
+        ctx, f_op, t_op, out_shape + (f_op.nrow, f_op.ncol), np.float32,
+        lambda out: ctx.seeps_maps(
+            f_op.addr, t_op.addr, wet_op.addr, p1_dev, tabs[0].size // ngroup,
+            ngroup, *tabs, f_op.nrow, f_op.ncol, f_op.row_stride,
+            wet_op.row_stride, np.float32(dry_threshold), np.float32(min_p1),
+            np.float32(max_p1), skipna, out))
+  return maps, out_dims + _map_dims(f_op)
+
+
+def run_rank_histogram(ctx: _lib.Context, x_op: Operand, t_op: Operand,
+                       ens_dim: str, nbins: int, reduce_dim: Optional[str],
+                       random_ties: bool, seed: int):
+  """Runs K10 for one variable.  Returns (hist[..., nrow, ncol, nbins], dims
+  without `bins`)."""
+  _check_truth(t_op, ens_dim)
+  with Staging(ctx) as stage:
+    x_op, t_op = stage.upload(x_op), stage.upload(t_op)
+    x_op, nmember, stride = split_member_dim(x_op, ens_dim)
+    _check_grid([x_op, t_op])
+    dims, shape, out_dims, out_shape, ngroup = _reduce_last(
+        *broadcast_dims(x_op, t_op), reduce_dim)
+    off_x, off_t = (offset_table(op, dims, shape) for op in (x_op, t_op))
+    hist = _run_maps(
+        ctx, x_op, t_op, out_shape + (x_op.nrow, x_op.ncol, nbins), np.float32,
+        lambda out: ctx.rank_histogram(
+            x_op.addr, t_op.addr, nmember, stride, off_x.size // ngroup,
+            ngroup, off_x, off_t, x_op.nrow, x_op.ncol, x_op.row_stride, nbins,
+            random_ties, seed, out))
+  return hist, out_dims + _map_dims(x_op)

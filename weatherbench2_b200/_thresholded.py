@@ -17,7 +17,6 @@ from weatherbench2_b200 import metrics as m
 from weatherbench2_b200 import thresholds as thr_lib
 from weatherbench2_b200 import xarray_lite as xl
 
-LAT, LON = sp.LAT, sp.LON
 # slots of the K7 output (include/wb2b200.h)
 _BRIER, _DEBIASED, _IGNORANCE, _RPS = 0, 1, 2, 3
 _GCRPS, _GVAR = 0, 1
@@ -49,13 +48,6 @@ def _threshold_spec(thresholds: t.Sequence, truth: xl.Dataset, name: str,
 def _quantile_coords(thresholds):
   return xl.Coord(('quantile',), np.asarray([th.quantile for th in thresholds],
                                             dtype=np.float64))
-
-
-def _region_list(region):
-  b = m._batch  # pylint: disable=protected-access
-  if b.active and m._region_index(region, b.regions) >= 0:  # pylint: disable=protected-access
-    return b.regions, m._region_index(region, b.regions), True  # pylint: disable=protected-access
-  return [region], 0, False
 
 
 def _stats_to_dataset(res: dict, slot: int, quantile_coord, sum_quantile: bool,
@@ -109,17 +101,12 @@ def _gaussian_stats(forecast: xl.Dataset, truth: xl.Dataset, thresholds,
 
 
 def _gaussian_request(forecast, truth, thresholds, region, skipna) -> dict:
-  regions, ri, cached = _region_list(region)
-  if cached:
-    b = m._batch  # pylint: disable=protected-access
-    key = ('gauss', id(forecast), id(truth), bool(skipna),
-           None if thresholds is None else tuple(id(th) for th in thresholds))
-    if key not in b.cache:
-      b.cache[key] = (_gaussian_stats(forecast, truth, thresholds, regions,
-                                      skipna), forecast, truth, thresholds)
-    res = b.cache[key][0]
-  else:
-    res = _gaussian_stats(forecast, truth, thresholds, regions, skipna)
+  res, ri = m._region_request(  # pylint: disable=protected-access
+      ('gauss', id(forecast), id(truth), bool(skipna),
+       None if thresholds is None else tuple(id(th) for th in thresholds)),
+      (forecast, truth, thresholds),
+      lambda regions: _gaussian_stats(forecast, truth, thresholds, regions,
+                                      skipna), region)
   return {k: (st[..., ri, :], dims, coords)
           for k, (st, dims, coords) in res.items()}
 
@@ -207,13 +194,8 @@ def _ens_threshold_stats(forecast: xl.Dataset, truth: xl.Dataset, ens_dim: str,
   ctx = m._context()  # pylint: disable=protected-access
   lat, lon = m._lat_lon(forecast)  # pylint: disable=protected-access
   out = {}
-  for name in m._common_vars(forecast, truth):  # pylint: disable=protected-access
-    f_da, t_da = forecast[name], truth[name]
-    if LAT not in f_da.dims or LON not in f_da.dims:
-      continue
-    f_da, t_da = xl.align_inner(f_da, t_da)
-    x_op = sp.prepare_operand(f_da, None, np.float32)
-    t_op = sp.prepare_operand(t_da, x_op.layout, np.float32)
+  for name, f_da, t_da, x_op, t_op in m._paired_operands(  # pylint: disable=protected-access
+      forecast, truth, np.float32):
     spec = _threshold_spec(thresholds, truth, name, t_da, x_op.layout)
     st, dims, _ = sp.run_ens_threshold_metrics(
         ctx, x_op, t_op, ens_dim, spec, lat, lon, regions, skipna,
@@ -226,19 +208,13 @@ def _ens_threshold_stats(forecast: xl.Dataset, truth: xl.Dataset, ens_dim: str,
 
 def _ens_threshold_request(forecast, truth, ens_dim, thresholds, region,
                            skipna) -> dict:
-  regions, ri, cached = _region_list(region)
-  if cached:
-    b = m._batch  # pylint: disable=protected-access
-    key = ('ensthr', id(forecast), id(truth), ens_dim, bool(skipna),
-           tuple(id(th) for th in thresholds))
-    if key not in b.cache:
-      b.cache[key] = (_ens_threshold_stats(forecast, truth, ens_dim,
+  res, ri = m._region_request(  # pylint: disable=protected-access
+      ('ensthr', id(forecast), id(truth), ens_dim, bool(skipna),
+       tuple(id(th) for th in thresholds)),
+      (forecast, truth, thresholds),
+      lambda regions: _ens_threshold_stats(forecast, truth, ens_dim,
                                            thresholds, regions, skipna),
-                      forecast, truth, thresholds)
-    res = b.cache[key][0]
-  else:
-    res = _ens_threshold_stats(forecast, truth, ens_dim, thresholds, regions,
-                               skipna)
+      region)
   return {k: (st[..., ri, :], dims, coords)
           for k, (st, dims, coords) in res.items()}
 
@@ -311,13 +287,8 @@ class _SpatialEnsembleThresholdMetric(_EnsembleThresholdMetric):
     ctx = m._context()  # pylint: disable=protected-access
     thresholds = list(self.thresholds)
     out = xl.Dataset(attrs=self._attrs())
-    for name in m._common_vars(forecast, truth):  # pylint: disable=protected-access
-      f_da, t_da = forecast[name], truth[name]
-      if LAT not in f_da.dims or LON not in f_da.dims:
-        continue
-      f_da, t_da = xl.align_inner(f_da, t_da)
-      x_op = sp.prepare_operand(f_da, None, np.float32)
-      t_op = sp.prepare_operand(t_da, x_op.layout, np.float32)
+    for name, f_da, t_da, x_op, t_op in m._paired_operands(  # pylint: disable=protected-access
+        forecast, truth, np.float32):
       spec = _threshold_spec(thresholds, truth, name, t_da, x_op.layout)
       maps, dims, _ = sp.run_ens_threshold_maps(
           ctx, x_op, t_op, self.ensemble_dim, spec, self._SLOT, reduce_dim,

@@ -83,6 +83,30 @@ def _region_index(region, regions) -> int:
   return -1
 
 
+def _batch_index(region) -> int:
+  """Index of `region` among the regions of the active `batch()`; -1 outside
+  a batch or for another region."""
+  return _region_index(region, _batch.regions) if _batch.active else -1
+
+
+def _batch_cached(key, keep, compute):
+  """`compute()`, evaluated once per `key` inside the active `batch()`.  The
+  cache entry holds `keep` alive: the objects whose ids make up the key."""
+  if key not in _batch.cache:
+    _batch.cache[key] = (compute(), keep)
+  return _batch.cache[key][0]
+
+
+def _region_request(key, keep, compute, region):
+  """(result, index of `region` in it): `compute(regions)` for all regions of
+  the active `batch()`, cached under `key`, when `region` is one of them;
+  else `compute([region])`."""
+  ri = _batch_index(region)
+  if ri < 0:
+    return compute([region]), 0
+  return _batch_cached(key, keep, lambda: compute(_batch.regions)), ri
+
+
 def _context() -> _lib.Context:
   return _lib.default_context()
 
@@ -98,9 +122,25 @@ def _common_vars(forecast: xl.Dataset, truth: xl.Dataset) -> list[str]:
 def _lat_lon(ds: xl.Dataset):
   lat = np.asarray(ds['latitude'].values)
   lon = np.asarray(ds['longitude'].values)
-  sp._assert_increasing(  # same ValueError as metrics.py:35-37 via :48
-      sp._latitude_cell_bounds(np.deg2rad(lat)))
+  sp.lat_weights(lat)  # same ValueError as metrics.py:35-37 via :48
   return lat, lon
+
+
+def _paired_operands(forecast: xl.Dataset, truth: xl.Dataset,
+                     dtype: t.Optional[np.dtype] = None):
+  """Yields (name, f_da, t_da, f_op, t_op) for every variable of both datasets
+  that has latitude and longitude dims: forecast and truth aligned by label
+  (xarray arithmetic joins shared dimensions, inner join), the forecast
+  operand in `dtype` (None: its own float type), the truth in the forecast
+  operand's layout and dtype."""
+  for name in _common_vars(forecast, truth):
+    f_da, t_da = forecast[name], truth[name]
+    if LAT not in f_da.dims or LON not in f_da.dims:
+      continue
+    f_da, t_da = xl.align_inner(f_da, t_da)
+    f_op = sp.prepare_operand(f_da, None, dtype)
+    t_op = sp.prepare_operand(t_da, f_op.layout, f_op.dtype)
+    yield name, f_da, t_da, f_op, t_op
 
 
 def _result_coords(out_dims, *sources: xl.DataArray) -> dict:
@@ -179,20 +219,12 @@ def _det_stats(forecast: xl.Dataset, truth: xl.Dataset, climatology,
                regions: t.Sequence, skipna: bool) -> dict:
   """{var: (stats[..., R, 10], out_dims, coords)} for all common variables."""
   ctx = _context()
-  names = _common_vars(forecast, truth)
   lat, lon = _lat_lon(forecast)
   clim_chunk = None
   if climatology is not None:
     clim_chunk = _get_climatology_chunk(xl.from_xarray(climatology), truth)
   prepared = {}
-  for name in names:
-    f_da, t_da = forecast[name], truth[name]
-    if LAT not in f_da.dims or LON not in f_da.dims:
-      continue
-    # xarray arithmetic joins shared dimensions by label (inner join)
-    f_da, t_da = xl.align_inner(f_da, t_da)
-    f_op = sp.prepare_operand(f_da)
-    t_op = sp.prepare_operand(t_da, f_op.layout, f_op.dtype)
+  for name, f_da, t_da, f_op, t_op in _paired_operands(forecast, truth):
     if t_op.row_stride != f_op.row_stride or t_op.on_device != f_op.on_device:
       raise ValueError(
           f'{name}: forecast and truth must share memory space and row stride')
@@ -221,17 +253,13 @@ def _det_stats(forecast: xl.Dataset, truth: xl.Dataset, climatology,
 def _det_request(forecast, truth, region, skipna, climatology=None) -> dict:
   """Per-variable stats [..., 10] for one region (served from the batch cache
   when possible)."""
-  if _batch.active and _region_index(region, _batch.regions) >= 0:
-    clim = climatology if climatology is not None else _batch.climatology
-    key = ('det', id(forecast), id(truth), id(clim), bool(skipna))
-    if key not in _batch.cache:
-      _batch.cache[key] = (_det_stats(forecast, truth, clim, _batch.regions,
-                                      skipna), forecast, truth, clim)
-    res = _batch.cache[key][0]
-    ri = _region_index(region, _batch.regions)
-  else:
-    res = _det_stats(forecast, truth, climatology, [region], skipna)
-    ri = 0
+  if climatology is None and _batch_index(region) >= 0:
+    climatology = _batch.climatology
+  res, ri = _region_request(
+      ('det', id(forecast), id(truth), id(climatology), bool(skipna)),
+      (forecast, truth, climatology),
+      lambda regions: _det_stats(forecast, truth, climatology, regions,
+                                 skipna), region)
   return {k: (st[..., ri, :], dims, coords)
           for k, (st, dims, coords) in res.items()}
 
@@ -320,43 +348,34 @@ def _wind_vector_stat(forecast, truth, u_name, v_name, region, skipna):
   ctx = _context()
   lat, lon = _lat_lon(forecast)
   das = [forecast[u_name], forecast[v_name], truth[u_name], truth[v_name]]
-  staged = []
-  fu = sp.prepare_operand(das[0])
-  ops = [fu] + [sp.prepare_operand(d, fu.layout, fu.dtype) for d in das[1:]]
-  if not fu.on_device:
-    # the vector kernel has no streaming host entry: stage contiguous copies
-    ops = []
-    for d in das:
-      arr = np.ascontiguousarray(d.values)
-      op = sp.prepare_operand(xl.DataArray(arr, d.dims),
-                              ops[0].layout if ops else None,
-                              ops[0].dtype if ops else None)
-      dptr = ctx.to_device(np.ascontiguousarray(op.data))
-      staged.append(dptr)
-      ops.append(dataclasses.replace(op, addr=dptr, on_device=True))
-    fu = ops[0]
-  for op in ops[1:]:
-    if _group_key(op) != _group_key(fu):
-      raise ValueError('wind components must share dtype, layout and device')
-  fu_op, fv_op, tu_op, tv_op = ops
-  dims, shape = sp.broadcast_dims(fu_op, tu_op, fv_op, tv_op)
-  base = min(op.addr for op in ops)
-  es = fu.itemsize
-  tabs = [sp.offset_table(op, dims, shape) + (op.addr - base) // es
-          for op in ops]
-  nfield = tabs[0].size
-  dtype_code = _lib.F32 if fu.dtype == np.float32 else _lib.F64
-  _, spec = sp.build_weights(ctx, lat, lon, [region], fu.layout,
-                             fu.row_stride, _global_cell_cache)[0]
-  out_dev = ctx.malloc(nfield * _lib.DET_NSTAT * 8)
-  try:
-    ctx.det_metrics_vector(base, base, base, base, dtype_code, tabs[0],
-                           tabs[1], tabs[2], tabs[3], spec, skipna, out_dev)
-    st = ctx.from_device(out_dev, (nfield, 1, _lib.DET_NSTAT), np.float64)
-  finally:
-    ctx.free(out_dev)
-    for p in staged:
-      ctx.free(p)
+  with sp.Staging(ctx) as stage:
+    fu = sp.prepare_operand(das[0])
+    ops = [fu] + [sp.prepare_operand(d, fu.layout, fu.dtype) for d in das[1:]]
+    if not fu.on_device:
+      # the vector kernel has no streaming host entry: stage contiguous copies
+      ops = []
+      for d in das:
+        arr = np.ascontiguousarray(d.values)
+        op = sp.prepare_operand(xl.DataArray(arr, d.dims),
+                                ops[0].layout if ops else None,
+                                ops[0].dtype if ops else None)
+        dptr = stage.array(np.ascontiguousarray(op.data))
+        ops.append(dataclasses.replace(op, addr=dptr, on_device=True))
+      fu = ops[0]
+    for op in ops[1:]:
+      if _group_key(op) != _group_key(fu):
+        raise ValueError('wind components must share dtype, layout and device')
+    fu_op, fv_op, tu_op, tv_op = ops
+    dims, shape = sp.broadcast_dims(fu_op, tu_op, fv_op, tv_op)
+    base, tabs = sp.addressing(ops, dims, shape)
+    dtype_code = _lib.F32 if fu.dtype == np.float32 else _lib.F64
+    groups = sp.build_weights(ctx, lat, lon, [region], fu.layout,
+                              fu.row_stride, _global_cell_cache)
+    st = sp.run_region_groups(
+        ctx, groups, (tabs[0].size, 1, _lib.DET_NSTAT), 1,
+        lambda w, out: ctx.det_metrics_vector(base, base, base, base,
+                                              dtype_code, *tabs, w, skipna,
+                                              out))
   st = st.reshape(shape + (_lib.DET_NSTAT,))
   coords = _result_coords(dims, das[0], das[2])
   return xl.DataArray(_ratio(st[..., 0], st[..., 6]), dims, coords)
@@ -480,13 +499,7 @@ class _SpatialDetMetric(Metric):
     forecast, truth, native = _prep(forecast, truth)
     ctx = _context()
     out = xl.Dataset()
-    for name in _common_vars(forecast, truth):
-      f_da, t_da = forecast[name], truth[name]
-      if LAT not in f_da.dims or LON not in f_da.dims:
-        continue
-      f_da, t_da = xl.align_inner(f_da, t_da)
-      f_op = sp.prepare_operand(f_da)
-      t_op = sp.prepare_operand(t_da, f_op.layout, f_op.dtype)
+    for name, f_da, t_da, f_op, t_op in _paired_operands(forecast, truth):
       maps, dims = sp.run_det_maps(ctx, f_op, t_op, self._STAT, reduce_dim,
                                    skipna)
       out[name] = xl.DataArray(maps, dims, _map_coords(dims, f_da, t_da), name)
