@@ -679,6 +679,53 @@ def bench_column_integral(args):
            q.numel(), 'cells', dict(card, run=run))
 
 
+def bench_thermo(args):
+  """Device-resident 0.25-degree (time=4, level=37, 721, 1440) float32 data:
+  the lapse rate (T and Z read, the float32 result written: 12 B per cell) and
+  the relative humidity on int64 levels (T and q read, the float64 result
+  written: 16 B per cell), in the (latitude, longitude) and (longitude,
+  latitude) layouts and with the level axis innermost, next to a device copy
+  measured in the same run; all of it twice."""
+  torch, _lib, ctx = setup()
+  from weatherbench2_b200 import _derived_wind as dw
+  card = _card()
+  level = np.array([1, 2, 3, 5, 7, 10, 20, 30, 50, 70, 100, 125, 150, 175,
+                    200, 225, 250, 300, 350, 400, 450, 500, 550, 600, 650,
+                    700, 750, 775, 800, 825, 850, 875, 900, 925, 950, 975,
+                    1000])
+  nouter, nlev, ncell = 4, level.size, NLAT * NLON
+  coef, uniform = dw.gradient_table(level)
+  pressure = level.astype(np.float64)
+  gen = torch.Generator(device='cuda').manual_seed(0)
+  n = nouter * nlev * ncell
+  t = torch.empty(n, device='cuda').normal_(250, 20, generator=gen)
+  z = torch.empty(n, device='cuda').normal_(5e4, 3e4, generator=gen)
+  q = torch.empty(n, device='cuda').uniform_(0, 0.02, generator=gen)
+  out = torch.empty(n, device='cuda')
+  out64 = torch.empty(n, device='cuda', dtype=torch.float64)
+  # (nouter, nlev, ninner) of each layout: both spatial layouts give the
+  # entries the same sizes; level innermost makes every column contiguous
+  layouts = [('(latitude, longitude)', nouter, nlev, ncell),
+             ('(longitude, latitude)', nouter, nlev, ncell),
+             ('level innermost', nouter * ncell, nlev, 1)]
+  copy = torch.empty_like(t)
+  for run in (1, 2):  # twice in one process, to show the spread
+    for name, no, nl, ni in layouts:
+      ms = timeit(lambda no=no, nl=nl, ni=ni: ctx.lapse_rate(
+          _lib.F32, t.data_ptr(), z.data_ptr(), no, nl, ni, coef, uniform,
+          out.data_ptr()), args.steps)
+      report(f'lapse_rate {name} 4x37x721x1440', ms, n * 12, n, 'cells',
+             dict(card, run=run))
+      ms = timeit(lambda no=no, nl=nl, ni=ni: ctx.relative_humidity(
+          _lib.F32, _lib.F64, t.data_ptr(), q.data_ptr(), no, nl, ni,
+          pressure, out64.data_ptr()), args.steps)
+      report(f'relative_humidity float32 -> float64 {name} 4x37x721x1440', ms,
+             n * 16, n, 'cells', dict(card, run=run))
+    ms = timeit(lambda: copy.copy_(t), args.steps)
+    report('device copy 4x37x721x1440 (torch copy_)', ms, n * 8, n, 'cells',
+           dict(card, run=run))
+
+
 def precip_bytes(nouter, ntime, ninner, window, esize=4, block=256):
   """Bytes a precipitation accumulation needs: the input read once plus the
   `window` halo rows each block of `block` outputs stages again, and the
@@ -954,7 +1001,8 @@ if __name__ == '__main__':
                            'maps', 'threshold', 'climatology',
                            'climatology_quantile', 'resample',
                            'wind_dynamics', 'precip_accumulation',
-                           'column_integral', 'quantile', 'average'])
+                           'column_integral', 'thermo', 'quantile',
+                           'average'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -968,5 +1016,6 @@ if __name__ == '__main__':
    'wind_dynamics': bench_wind_dynamics,
    'precip_accumulation': bench_precip_accumulation,
    'column_integral': bench_column_integral,
+   'thermo': bench_thermo,
    'quantile': bench_quantile,
    'average': bench_average}[a.kernel](a)

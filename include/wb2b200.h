@@ -390,6 +390,76 @@ int wb2_column_integral(wb2_ctx* ctx, int kind, int dtype, const void* q, const 
                         int64_t ninner, int32_t nlon, int64_t lon_stride,
                         const double* weight, void* out);
 
+/* wb2_lapse_rate replaces LapseRate.compute (derived_variables.py:355-362):
+ *   dT_dp / dz_dp,  dT_dp = T.differentiate('level'),
+ *   dz_dp = (1 / 9.81) * Z.differentiate('level').
+ * t, z    device arrays of `dtype` (WB2_F32 / WB2_F64) [nouter][nlev][ninner]:
+ *         temperature and geopotential in the same layout, the level axis
+ *         wherever it sits (ninner = 1 when it is innermost);
+ * coef    host [nlev][3] float64, np.gradient's coefficients along the level
+ *         coordinate as _derived_wind.gradient_table gives them (the layout of
+ *         wb2_wind_dynamics' lat_coef), `uniform` != 0 when every level step
+ *         equals the first exactly;
+ * out     device [nouter][nlev][ninner] of `dtype`.
+ * One thread per (outer, inner) column walks its levels; consecutive threads
+ * take consecutive inner cells.  With ninner < 32 (the level axis innermost)
+ * one thread per cell reads its stencil instead, so a warp's loads stay
+ * contiguous; the arithmetic is the same.  Numerics, with T the data type and every step
+ * a correctly rounded operation (no FMA contraction):
+ *   dT, dZ  np.gradient(f, level, edge_order=1) rounded once to T: the edges
+ *           T(f[1] - f[0]) / dx[0] and T(f[n-1] - f[n-2]) / dx[n-2] and the
+ *           uniform interior T(f[k+1] - f[k-1]) / (2 dx) as float64 divisions,
+ *           the non-uniform interior (a f[k-1] + b f[k]) + c f[k+1] in float64;
+ *   dz      T(1/9.81) * dZ in T (the Python scalar is weak under NEP 50);
+ *   out     dT / dz in T.
+ * For float32 and float64 data on an integer or float64 level coordinate this is
+ * the reference's result bit for bit, NaN and +-inf included (dz == 0 gives
+ * +-inf or NaN, as NumPy does).  Deviations: the caller casts integer data to
+ * float64 (np.gradient does the same) and T and Z of different float types to
+ * their common type (the reference would differentiate each in its own type);
+ * a float32 level coordinate is taken as float64.  Errors: NULL operands,
+ * negative sizes, an unknown dtype, nlev < 2.  One kernel launch per call.      */
+int wb2_lapse_rate(wb2_ctx* ctx, int dtype, const void* t, const void* z, int64_t nouter,
+                   int32_t nlev, int64_t ninner, const double* coef, int uniform,
+                   void* out);
+
+/* wb2_relative_humidity replaces RelativeHumidity.compute
+ * (derived_variables.py:450-468), MetPy's formula with Bolton's (1980)
+ * saturation vapour pressure, T in K and p in hPa:
+ *   svp = 6.112 * exp(17.67 * (T - 273.15) / (T - 29.65))
+ *   mr  = q / (1 - q)
+ *   out = mr / (0.622 * svp / (p - svp))
+ * t, q      device arrays of `dtype` (WB2_F32 / WB2_F64) [nouter][npres][ninner],
+ *           temperature and specific humidity in the same layout;
+ * pressure  host [npres] float64: the pressure coordinate along the npres axis
+ *           (npres = 1 for a scalar coordinate), in the coordinate's own values;
+ * out       device [nouter][npres][ninner] of `out_dtype`, which the caller sets
+ *           to NumPy's promotion of the pressure coordinate's dtype with the
+ *           data's (int64 levels and float32 data give float64, float32 levels
+ *           float32); float64 data with a float32 out_dtype is rejected.
+ * Long slabs (ninner >= 256) run one CTA row per (outer, p) slab, so the
+ * pressure is uniform within a CTA; shorter ones a flat loop.  Numerics, with T
+ * the data type and O = out_dtype, every step correctly rounded, no FMA
+ * contraction, in the reference's dtypes:
+ *   x    T(17.67) * (t - T(273.15)) / (t - T(29.65)) in T;
+ *   e    exp(x): a float32 x is evaluated in float64 and rounded once to float32;
+ *        a float64 x takes CUDA's exp, at most 1 ulp from the exact value;
+ *   svp  T(6.112) * e in T;   mr = q / (T(1) - q) in T;
+ *   out  O(T(0.622) * svp) / (O(p) - O(svp)), then O(mr) / that, in O.
+ * NaN and +-inf propagate as in NumPy.  The gap to the reference is NumPy's own
+ * exp error: its float32 exp (the AVX512F path of NumPy 2.3) lies up to 2 ulp
+ * from the correctly rounded value over every float32 T in [180, 330] K, so svp
+ * differs by at most 3 float32 ulp and |out - ref| <= 2^-20 |ref| (1 + |svp / (p -
+ * svp)|); for float64 data both exps are within 1 ulp, and the bound is
+ * 2^-49 |ref| (1 + |svp / (p - svp)|).  Deviations: the caller casts integer data
+ * to float64 (NumPy's result is the same) and t and q of different float types to
+ * their common type (the reference computes svp in t's type and mr in q's).
+ * Errors: NULL operands, negative sizes, npres < 1, an unknown dtype or
+ * out_dtype.  One kernel launch per call.                                        */
+int wb2_relative_humidity(wb2_ctx* ctx, int dtype, int out_dtype, const void* t,
+                          const void* q, int64_t nouter, int32_t npres, int64_t ninner,
+                          const double* pressure, void* out);
+
 /* wb2_ens_mean replaces the ensemble-mean pipeline of
  * scripts/compute_ensemble_mean.py:110-141 (xbeam.Mean(realization, skipna)):
  * out[field][cell] = mean_m x[off_x[field] + m * member_stride + cell], float32;

@@ -1,0 +1,241 @@
+"""Thermodynamic derived variables -- same classes as
+weatherbench2/derived_variables.py:341-362 and 433-468: the lapse rate and the
+relative humidity, computed on the device (csrc/thermo.cu).  Imported into
+`weatherbench2_b200.derived_variables`.
+
+CUDA input gives a CUDA tensor on the same device, which the metric kernels
+read in place; NumPy, memmap or lazily gathered input is read once as NumPy
+and gives NumPy; native xarray gives native xarray.  An operand in another dim
+order is permuted to the order of the one whose dims the result takes:
+temperature's for the lapse rate, specific humidity's for the relative
+humidity, as xarray's `dT_dp / dz_dp` and `mixing_ratio / smr` order them.
+Operands whose dims or sizes differ raise ValueError, where xarray would align
+them.  Numerics and deviations: include/wb2b200.h and DESIGN.md section 8i.
+"""
+from __future__ import annotations
+
+import dataclasses
+import typing as t
+
+import numpy as np
+
+from weatherbench2_b200 import _derived_wind
+from weatherbench2_b200 import _lib
+from weatherbench2_b200 import derived_variables as dv
+from weatherbench2_b200 import xarray_lite as xl
+
+
+def _operands(ds, names):
+  """The named variables (KeyError for a missing one), each as a CUDA tensor
+  or NumPy array, and their common float dtype: integers are taken as float64,
+  as np.gradient and NumPy's arithmetic take them."""
+  das = [ds[n] for n in names]
+  for name, da in zip(names[1:], das[1:]):
+    if set(da.dims) != set(das[0].dims) or any(
+        da.sizes[d] != das[0].sizes[d] for d in das[0].dims):
+      raise ValueError(f'{names[0]!r} and {name!r} differ in dims or shape')
+  datas = [da.data if xl._is_torch(da.data) and da.data.is_cuda  # pylint: disable=protected-access
+           else xl._np(da.data) for da in das]  # pylint: disable=protected-access
+  dtypes = []
+  for name, x in zip(names, datas):
+    try:
+      dtype = np.dtype(str(x.dtype).replace('torch.', ''))
+    except TypeError:
+      dtype = None
+    if dtype is not None and dtype.kind in 'iu':
+      dtype = np.dtype(np.float64)
+    if dtype not in (np.float32, np.float64):
+      raise TypeError(f'variable {name!r} has dtype {x.dtype}: the lapse rate '
+                      'and relative humidity take float32, float64 or integer '
+                      'data')
+    dtypes.append(dtype)
+  return das, datas, np.result_type(*dtypes)
+
+
+def _run(datas, das, dims, dtype, out_dtype, call):
+  """Permutes every operand to `dims`, runs `call(ptrs, out)` once and returns
+  the result data: a CUDA tensor when an operand is one, else NumPy."""
+  shape = tuple(das[0].sizes[d] for d in dims)
+  perms = [None if da.dims == dims else tuple(da.dims.index(d) for d in dims)
+           for da in das]
+  ctx = _lib.default_context()
+  first = next((x for x in datas if xl._is_torch(x)), None)  # pylint: disable=protected-access
+  if first is not None:  # _operands left only CUDA tensors as torch
+    import torch  # pylint: disable=import-outside-toplevel
+    tdtype = getattr(torch, np.dtype(dtype).name)
+    xs = []
+    for x, perm in zip(datas, perms):
+      if not xl._is_torch(x):  # pylint: disable=protected-access
+        x = torch.from_numpy(np.asarray(x))
+      if perm is not None:
+        x = x.permute(*perm)
+      xs.append(x.to(first.device, tdtype).contiguous())
+    out = torch.empty(shape, device=first.device,
+                      dtype=getattr(torch, np.dtype(out_dtype).name))
+    if out.numel():
+      torch.cuda.current_stream(first.device).synchronize()
+      call([x.data_ptr() for x in xs], out.data_ptr())
+      ctx.synchronize()
+    return out
+  xs = [np.ascontiguousarray(
+      xl._np(x) if perm is None else np.transpose(xl._np(x), perm),  # pylint: disable=protected-access
+      dtype=dtype) for x, perm in zip(datas, perms)]
+  n = int(np.prod(shape, dtype=np.int64))
+  if not n:
+    return np.zeros(shape, out_dtype)
+  ptrs, po = [], None
+  try:
+    for x in xs:
+      ptrs.append(ctx.to_device(x))
+    po = ctx.malloc(n * np.dtype(out_dtype).itemsize)
+    call(ptrs, po)
+    return ctx.from_device(po, shape, out_dtype)
+  finally:
+    for p in ptrs + ([po] if po else []):
+      ctx.free(p)
+
+
+def _split(shape, axis):
+  """(nouter, n, ninner) of `shape` around `axis`."""
+  nouter = int(np.prod(shape[:axis], dtype=np.int64))
+  ninner = int(np.prod(shape[axis + 1:], dtype=np.int64))
+  return nouter, shape[axis], ninner
+
+
+def _result(data, dims, coords, native):
+  result = xl.DataArray(data, dims, coords)
+  if native:
+    return xl.to_xarray(xl.Dataset({'_': result}))['_']
+  return result
+
+
+def lapse_rate(dataset, temperature_name: str, geopotential_name: str):
+  """One wb2_lapse_rate call: dT/dlevel / ((1 / 9.81) dZ/dlevel) with
+  np.gradient's arithmetic along `level`, in temperature's dims."""
+  native = xl.is_native_xarray(dataset)
+  ds = xl.from_xarray(dataset)
+  names = [temperature_name, geopotential_name]
+  das, datas, dtype = _operands(ds, names)
+  temp = das[0]
+  if 'level' not in temp.dims:
+    raise ValueError(f'{temperature_name!r} has no "level" dimension')
+  level = (temp.coords['level'] if 'level' in temp.coords
+           else ds.coords.get('level'))
+  if level is None or tuple(level.dims) != ('level',):
+    raise ValueError('Coordinate level does not exist.')
+  coef, uniform = _derived_wind.gradient_table(level.values)  # ValueError: < 2
+  dims = temp.dims
+  shape = tuple(temp.sizes[d] for d in dims)
+  nouter, nlev, ninner = _split(shape, dims.index('level'))
+  code = _lib.F64 if dtype == np.float64 else _lib.F32
+  ctx = _lib.default_context()
+
+  def call(ptrs, out):
+    ctx.lapse_rate(code, ptrs[0], ptrs[1], nouter, nlev, ninner, coef, uniform,
+                   out)
+
+  data = _run(datas, das, dims, dtype, dtype, call)
+  coords = dict(das[1].coords)
+  coords.update(temp.coords)
+  return _result(data, dims, coords, native)
+
+
+def relative_humidity(dataset, temperature_name: str,
+                      specific_humidity_name: str, pressure_name: str):
+  """One wb2_relative_humidity call: MetPy's relative humidity from specific
+  humidity with Bolton's saturation vapour pressure, T in K and the pressure
+  coordinate in hPa, in specific humidity's dims."""
+  native = xl.is_native_xarray(dataset)
+  ds = xl.from_xarray(dataset)
+  names = [specific_humidity_name, temperature_name]  # q first: its dims
+  das, datas, dtype = _operands(ds, names)
+  q = das[0]
+  if pressure_name not in ds.coords:
+    raise KeyError(pressure_name)
+  pcoord = ds.coords[pressure_name]
+  pvalues = np.asarray(pcoord.values)
+  if len(pcoord.dims) > 1:
+    raise ValueError(f'pressure coordinate {pressure_name!r} has dims '
+                     f'{pcoord.dims}: relative humidity takes a scalar or '
+                     'one-dimensional pressure coordinate')
+  if pcoord.dims and pcoord.dims[0] not in q.dims:
+    raise ValueError(f'pressure coordinate {pressure_name!r} lies along '
+                     f'{pcoord.dims[0]!r}, which {specific_humidity_name!r} '
+                     'lacks; relative humidity does not broadcast it')
+  if pvalues.dtype.kind not in 'iuf':
+    raise TypeError(f'pressure coordinate {pressure_name!r} has dtype '
+                    f'{pvalues.dtype}')
+  out_dtype = np.result_type(pvalues.dtype, dtype)
+  if out_dtype not in (np.float32, np.float64):
+    raise TypeError(f'pressure coordinate {pressure_name!r} of dtype '
+                    f'{pvalues.dtype} promotes the result to {out_dtype}')
+  dims = q.dims
+  shape = tuple(q.sizes[d] for d in dims)
+  if pcoord.dims:
+    nouter, npres, ninner = _split(shape, dims.index(pcoord.dims[0]))
+  else:
+    nouter, npres, ninner = 1, 1, int(np.prod(shape, dtype=np.int64))
+  pressure = pvalues.astype(np.float64).reshape(-1)
+  code = _lib.F64 if dtype == np.float64 else _lib.F32
+  out_code = _lib.F64 if out_dtype == np.float64 else _lib.F32
+  ctx = _lib.default_context()
+
+  def call(ptrs, out):
+    ctx.relative_humidity(code, out_code, ptrs[1], ptrs[0], nouter, npres,
+                          ninner, pressure, out)
+
+  data = _run(datas, das, dims, dtype, out_dtype, call)
+  coords = dict(das[1].coords)
+  coords.update(q.coords)
+  if pressure_name not in coords:
+    coords[pressure_name] = pcoord
+  return _result(data, dims, coords, native)
+
+
+@dataclasses.dataclass
+class LapseRate(dv.DerivedVariable):
+  """Lapse rate in temperature, dT/dp / dz/dp with z = Z / 9.81
+  (derived_variables.py:341-362).  Needs a `level` dimension and coordinate
+  with at least 2 levels."""
+
+  temperature_name: str = 'temperature'
+  geopotential_name: str = 'geopotential'
+
+  @property
+  def base_variables(self) -> list[str]:
+    return [self.temperature_name, self.geopotential_name]
+
+  @property
+  def core_dims(self) -> t.Tuple[t.Tuple[t.List[str], ...], t.List[str]]:
+    return (['level'], ['level']), ['level']
+
+  def compute(self, dataset):
+    return lapse_rate(dataset, self.temperature_name, self.geopotential_name)
+
+
+@dataclasses.dataclass
+class RelativeHumidity(dv.DerivedVariable):
+  """Relative humidity from specific humidity (derived_variables.py:433-468),
+  MetPy's relative_humidity_from_specific_humidity with Bolton's (1980)
+  saturation vapour pressure 6.112 exp(17.67 T / (T + 243.5)), T in degrees
+  Celsius.  Temperature is in K and the pressure coordinate in hPa."""
+
+  temperature_name: str = 'temperature'
+  specific_humidity_name: str = 'specific_humidity'
+  pressure_name: str = 'level'
+
+  @property
+  def base_variables(self) -> list[str]:
+    return [
+        self.temperature_name,
+        self.specific_humidity_name,
+        self.pressure_name,
+    ]
+
+  @property
+  def core_dims(self) -> t.Tuple[t.Tuple[t.List[str], ...], t.List[str]]:
+    return ([], []), []
+
+  def compute(self, dataset):
+    return relative_humidity(dataset, self.temperature_name,
+                             self.specific_humidity_name, self.pressure_name)

@@ -130,6 +130,12 @@ PROTOTYPES = {
     'wb2_column_integral': (C.c_int, [
         _P, C.c_int, C.c_int, _P, _P, _P, C.c_int64, C.c_int64, C.c_int32,
         C.c_int64, C.c_int32, C.c_int64, C.POINTER(C.c_double), _P]),
+    'wb2_lapse_rate': (C.c_int, [
+        _P, C.c_int, _P, _P, C.c_int64, C.c_int32, C.c_int64,
+        C.POINTER(C.c_double), C.c_int, _P]),
+    'wb2_relative_humidity': (C.c_int, [
+        _P, C.c_int, C.c_int, _P, _P, C.c_int64, C.c_int32, C.c_int64,
+        C.POINTER(C.c_double), _P]),
     'wb2_ens_mean': (C.c_int, [_P, _P, C.c_int32, C.c_int64, C.c_int64, _I64P,
                                C.c_int64, C.c_int, _P]),
     'wb2_spectrum_interp': (C.c_int, [_P, _P, C.c_int64, C.c_int32, C.c_int32,
@@ -669,6 +675,29 @@ class Context:
         int(nouter), int(outer_stride), int(nlev), int(ninner), int(nlon),
         int(lon_stride), _as_ptr(w, C.c_double), _P(out) if out else None))
     del w
+
+  def lapse_rate(self, dtype: int, t: int, z: int, nouter: int, nlev: int,
+                 ninner: int, coef: np.ndarray, uniform: bool, out: int):
+    """t / z / out are DEVICE addresses (wb2_lapse_rate); coef is the host
+    [nlev][3] float64 table of _derived_wind.gradient_table."""
+    c = np.ascontiguousarray(coef, dtype=np.float64)
+    check(self.lib.wb2_lapse_rate(
+        self.handle, int(dtype), _P(t) if t else None, _P(z) if z else None,
+        int(nouter), int(nlev), int(ninner), _as_ptr(c, C.c_double),
+        int(bool(uniform)), _P(out) if out else None))
+    del c
+
+  def relative_humidity(self, dtype: int, out_dtype: int, t: int, q: int,
+                        nouter: int, npres: int, ninner: int,
+                        pressure: np.ndarray, out: int):
+    """t / q / out are DEVICE addresses (wb2_relative_humidity); pressure is
+    the host [npres] float64 table of the pressure coordinate."""
+    p = np.ascontiguousarray(pressure, dtype=np.float64)
+    check(self.lib.wb2_relative_humidity(
+        self.handle, int(dtype), int(out_dtype), _P(t) if t else None,
+        _P(q) if q else None, int(nouter), int(npres), int(ninner),
+        _as_ptr(p, C.c_double), _P(out) if out else None))
+    del p
 
   def ens_mean(self, x: int, nmember: int, member_stride: int,
                off_x: np.ndarray, slab: int, skipna: bool, out: int):

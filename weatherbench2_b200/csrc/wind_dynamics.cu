@@ -29,6 +29,7 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "gradient.cuh"
 
 namespace wb2 {
 namespace {
@@ -54,20 +55,8 @@ struct DynParams {
   const double* pressure;  // [nlev]
 };
 
-// np.gradient(f, x, edge_order=1) at index i of an axis of n points, element
-// stride s, rounded to float32 as np.gradient stores it.
-__device__ __forceinline__ float gradient(const float* __restrict__ p, int i, int n, int64_t s,
-                                          const double* __restrict__ coef, bool uniform) {
-  const double* c = coef + 3 * i;
-  if (i == 0) return __double2float_rn(__ddiv_rn(double(__fsub_rn(__ldg(p + s), __ldg(p))), __ldg(c)));
-  if (i == n - 1)
-    return __double2float_rn(__ddiv_rn(double(__fsub_rn(__ldg(p), __ldg(p - s))), __ldg(c)));
-  const float fm = __ldg(p - s), fp = __ldg(p + s);
-  if (uniform) return __double2float_rn(__ddiv_rn(double(__fsub_rn(fp, fm)), __ldg(c)));
-  return __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn(__ldg(c), double(fm)),
-                                               __dmul_rn(__ldg(c + 1), double(__ldg(p)))),
-                                     __dmul_rn(__ldg(c + 2), double(fp))));
-}
+// np.gradient(f, x, edge_order=1) is gradient<float>() of gradient.cuh: each
+// derivative rounded to float32 as np.gradient stores it.
 
 // the reference's _d_dx (float64) and _d_dy (float32)
 __device__ __forceinline__ double d_dx(float g, double cos_lat) {

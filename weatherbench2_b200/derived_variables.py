@@ -10,8 +10,8 @@ csrc/resample.cu) and are re-exported here.  The column integrals over
 pressure level of derived_variables.py:212-228 and 365-430 -- eddy kinetic
 energy, total column water and integrated water transport -- live in
 _derived_column.py (csrc/column_integral.cu) and are re-exported here.  The
-remaining derived variables of the reference (lapse rate, relative humidity)
-are not reproduced.
+lapse rate and relative humidity of derived_variables.py:341-362 and 433-468
+live in _derived_thermo.py (csrc/thermo.cu) and are re-exported here.
 """
 from __future__ import annotations
 
@@ -307,15 +307,18 @@ from weatherbench2_b200._derived_precip import (  # noqa: E402  pylint: disable=
     AggregatePrecipitationAccumulation, PrecipitationAccumulation)
 from weatherbench2_b200._derived_column import (  # noqa: E402  pylint: disable=wrong-import-position
     EddyKineticEnergy, IntegratedWaterTransport, TotalColumnWater)
+from weatherbench2_b200._derived_thermo import (  # noqa: E402  pylint: disable=wrong-import-position
+    LapseRate, RelativeHumidity)
 
 # The named derived variables of weatherbench2/derived_variables.py:724-773 that
 # have a device implementation: wind speed, the horizontal-derivative family
 # (divergence, vorticity, vertical velocity, geostrophic and ageostrophic
 # winds), the column integrals (eddy kinetic energy, total column water,
 # integrated vapor transport) and the precipitation accumulations.  The
-# remaining entries of the reference's table (lapse rate, relative humidity)
-# are not reproduced; asking for one raises KeyError here instead of silently
-# running on the host.
+# reference's 'lapse_rate' and 'relative_humidity' entries are not registered
+# yet: their classes, LapseRate and RelativeHumidity, run on the device and
+# work anywhere a DerivedVariable is accepted, but asking this table for either
+# name raises KeyError until a follow-up adds the two entries.
 DERIVED_VARIABLE_DICT = {
     'wind_speed': WindSpeed(u_name='u_component_of_wind',
                             v_name='v_component_of_wind'),

@@ -598,10 +598,13 @@ class Dataset:
                if all(d in c.dims for d in v.dims)}
         return DataArray(c.values, c.dims, sub, key, c.attrs)
       raise KeyError(key)
-    missing = [k for k in key if k not in self._vars]
+    # a coordinate name may be listed, as in xarray: it stays a coordinate
+    # (RelativeHumidity lists its pressure coordinate among its base variables)
+    missing = [k for k in key if k not in self._vars and k not in self._coords]
     if missing:
       raise KeyError(missing)
-    return Dataset({k: self[k] for k in key}, self._coords, self.attrs)
+    return Dataset({k: self[k] for k in key if k in self._vars}, self._coords,
+                   self.attrs)
 
   def __getattr__(self, name):
     if name.startswith('_') or name == 'attrs':
