@@ -3,7 +3,7 @@ weatherbench2/derived_variables.py:212-228 and 365-430: total column water,
 integrated water transport and eddy kinetic energy, computed on the device
 (csrc/column_integral.cu).  Imported into `weatherbench2_b200.derived_variables`.
 
-CUDA input gives a CUDA tensor on the same device, which the metric kernels
+A CUDA operand gives a CUDA tensor on its device, which the metric kernels
 read in place; NumPy, memmap or lazily gathered input gives NumPy; native
 xarray gives native xarray.  Float32 data gives float32, float64 gives
 float64.  The result has the input's dims without `level`, in the same order,
@@ -19,6 +19,7 @@ import numpy as np
 
 from weatherbench2_b200 import _derived_wind
 from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import derived_variables as dv
 from weatherbench2_b200 import xarray_lite as xl
 
@@ -47,10 +48,7 @@ def column_integral(dataset, kind: int, names: t.Sequence[str],
       raise ValueError(f'{name!r} has no "level" dimension')
   if 'level' not in ref.coords:
     raise KeyError('level')
-  for name, da in zip(names[1:], das[1:]):
-    if set(da.dims) != set(ref.dims) or any(
-        da.sizes[d] != ref.sizes[d] for d in ref.dims):
-      raise ValueError(f'{names[0]!r} and {name!r} differ in dims or shape')
+  _derived_wind.check_same_grid(names, das)
   # CUDA tensors stay where they are; anything else is read once as NumPy
   datas = [da.data if xl._is_torch(da.data) and da.data.is_cuda  # pylint: disable=protected-access
            else xl._np(da.data) for da in das]  # pylint: disable=protected-access
@@ -97,41 +95,10 @@ def column_integral(dataset, kind: int, names: t.Sequence[str],
                (ptrs[0], ptrs[1], ptrs[2]) if kind == IVT else
                (None, ptrs[0], ptrs[1]))
     ctx.column_integral(kind, code, q, u, v, nouter, nlev * ninner, nsel,
-                        ninner, nlon, lon_stride, weight, out)
+                        ninner, nlon, lon_stride, weight, out[0])
 
-  first = datas[0]
-  if xl._is_torch(first) and first.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    tdtype = getattr(torch, np.dtype(dtype).name)
-    xs = []
-    for x, perm in zip(datas, perms):
-      if not xl._is_torch(x):  # pylint: disable=protected-access
-        x = torch.from_numpy(np.asarray(x))
-      if perm is not None:
-        x = x.permute(*perm)
-      xs.append(x.to(first.device, tdtype).contiguous())
-    data = torch.empty(out_shape, device=first.device, dtype=tdtype)
-    if data.numel():
-      torch.cuda.current_stream(first.device).synchronize()
-      call([x.data_ptr() for x in xs], data.data_ptr())
-      ctx.synchronize()
-  else:
-    xs = [np.ascontiguousarray(
-        xl._np(x) if perm is None else np.transpose(xl._np(x), perm),  # pylint: disable=protected-access
-        dtype=dtype) for x, perm in zip(datas, perms)]
-    if not int(np.prod(out_shape, dtype=np.int64)):
-      data = np.zeros(out_shape, dtype)
-    else:
-      ptrs, po = [], None
-      try:
-        for x in xs:
-          ptrs.append(ctx.to_device(x))
-        po = ctx.malloc(int(np.prod(out_shape)) * np.dtype(dtype).itemsize)
-        call(ptrs, po)
-        data = ctx.from_device(po, out_shape, dtype)
-      finally:
-        for p in ptrs + ([po] if po else []):
-          ctx.free(p)
+  data, = _streamed.run_whole(datas, [(out_shape, dtype)], call, perms=perms,
+                              dtype=dtype)
   out_dims = tuple(d for d in work if d != 'level')
   coords = {k: c for k, c in ref.coords.items() if 'level' not in c.dims}
   result = xl.DataArray(data, out_dims, coords)

@@ -3,7 +3,7 @@ weatherbench2/derived_variables.py:341-362 and 433-468: the lapse rate and the
 relative humidity, computed on the device (csrc/thermo.cu).  Imported into
 `weatherbench2_b200.derived_variables`.
 
-CUDA input gives a CUDA tensor on the same device, which the metric kernels
+A CUDA operand gives a CUDA tensor on its device, which the metric kernels
 read in place; NumPy, memmap or lazily gathered input is read once as NumPy
 and gives NumPy; native xarray gives native xarray.  An operand in another dim
 order is permuted to the order of the one whose dims the result takes:
@@ -21,19 +21,18 @@ import numpy as np
 
 from weatherbench2_b200 import _derived_wind
 from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import derived_variables as dv
 from weatherbench2_b200 import xarray_lite as xl
 
 
 def _operands(ds, names):
   """The named variables (KeyError for a missing one), each as a CUDA tensor
-  or NumPy array, and their common float dtype: integers are taken as float64,
-  as np.gradient and NumPy's arithmetic take them."""
+  or NumPy array, their permutations to the first one's dims (None for that
+  order), and their common float dtype: integers are taken as float64, as
+  np.gradient and NumPy's arithmetic take them."""
   das = [ds[n] for n in names]
-  for name, da in zip(names[1:], das[1:]):
-    if set(da.dims) != set(das[0].dims) or any(
-        da.sizes[d] != das[0].sizes[d] for d in das[0].dims):
-      raise ValueError(f'{names[0]!r} and {name!r} differ in dims or shape')
+  _derived_wind.check_same_grid(names, das)
   datas = [da.data if xl._is_torch(da.data) and da.data.is_cuda  # pylint: disable=protected-access
            else xl._np(da.data) for da in das]  # pylint: disable=protected-access
   dtypes = []
@@ -49,50 +48,10 @@ def _operands(ds, names):
                       'and relative humidity take float32, float64 or integer '
                       'data')
     dtypes.append(dtype)
-  return das, datas, np.result_type(*dtypes)
-
-
-def _run(datas, das, dims, dtype, out_dtype, call):
-  """Permutes every operand to `dims`, runs `call(ptrs, out)` once and returns
-  the result data: a CUDA tensor when an operand is one, else NumPy."""
-  shape = tuple(das[0].sizes[d] for d in dims)
+  dims = das[0].dims
   perms = [None if da.dims == dims else tuple(da.dims.index(d) for d in dims)
            for da in das]
-  ctx = _lib.default_context()
-  first = next((x for x in datas if xl._is_torch(x)), None)  # pylint: disable=protected-access
-  if first is not None:  # _operands left only CUDA tensors as torch
-    import torch  # pylint: disable=import-outside-toplevel
-    tdtype = getattr(torch, np.dtype(dtype).name)
-    xs = []
-    for x, perm in zip(datas, perms):
-      if not xl._is_torch(x):  # pylint: disable=protected-access
-        x = torch.from_numpy(np.asarray(x))
-      if perm is not None:
-        x = x.permute(*perm)
-      xs.append(x.to(first.device, tdtype).contiguous())
-    out = torch.empty(shape, device=first.device,
-                      dtype=getattr(torch, np.dtype(out_dtype).name))
-    if out.numel():
-      torch.cuda.current_stream(first.device).synchronize()
-      call([x.data_ptr() for x in xs], out.data_ptr())
-      ctx.synchronize()
-    return out
-  xs = [np.ascontiguousarray(
-      xl._np(x) if perm is None else np.transpose(xl._np(x), perm),  # pylint: disable=protected-access
-      dtype=dtype) for x, perm in zip(datas, perms)]
-  n = int(np.prod(shape, dtype=np.int64))
-  if not n:
-    return np.zeros(shape, out_dtype)
-  ptrs, po = [], None
-  try:
-    for x in xs:
-      ptrs.append(ctx.to_device(x))
-    po = ctx.malloc(n * np.dtype(out_dtype).itemsize)
-    call(ptrs, po)
-    return ctx.from_device(po, shape, out_dtype)
-  finally:
-    for p in ptrs + ([po] if po else []):
-      ctx.free(p)
+  return das, datas, perms, np.result_type(*dtypes)
 
 
 def _split(shape, axis):
@@ -115,7 +74,7 @@ def lapse_rate(dataset, temperature_name: str, geopotential_name: str):
   native = xl.is_native_xarray(dataset)
   ds = xl.from_xarray(dataset)
   names = [temperature_name, geopotential_name]
-  das, datas, dtype = _operands(ds, names)
+  das, datas, perms, dtype = _operands(ds, names)
   temp = das[0]
   if 'level' not in temp.dims:
     raise ValueError(f'{temperature_name!r} has no "level" dimension')
@@ -132,9 +91,10 @@ def lapse_rate(dataset, temperature_name: str, geopotential_name: str):
 
   def call(ptrs, out):
     ctx.lapse_rate(code, ptrs[0], ptrs[1], nouter, nlev, ninner, coef, uniform,
-                   out)
+                   out[0])
 
-  data = _run(datas, das, dims, dtype, dtype, call)
+  data, = _streamed.run_whole(datas, [(shape, dtype)], call,
+                              perms=perms, dtype=dtype)
   coords = dict(das[1].coords)
   coords.update(temp.coords)
   return _result(data, dims, coords, native)
@@ -148,7 +108,7 @@ def relative_humidity(dataset, temperature_name: str,
   native = xl.is_native_xarray(dataset)
   ds = xl.from_xarray(dataset)
   names = [specific_humidity_name, temperature_name]  # q first: its dims
-  das, datas, dtype = _operands(ds, names)
+  das, datas, perms, dtype = _operands(ds, names)
   q = das[0]
   if pressure_name not in ds.coords:
     raise KeyError(pressure_name)
@@ -182,9 +142,10 @@ def relative_humidity(dataset, temperature_name: str,
 
   def call(ptrs, out):
     ctx.relative_humidity(code, out_code, ptrs[1], ptrs[0], nouter, npres,
-                          ninner, pressure, out)
+                          ninner, pressure, out[0])
 
-  data = _run(datas, das, dims, dtype, out_dtype, call)
+  data, = _streamed.run_whole(datas, [(shape, out_dtype)], call,
+                              perms=perms, dtype=dtype)
   coords = dict(das[1].coords)
   coords.update(q.coords)
   if pressure_name not in coords:

@@ -6,10 +6,12 @@ weatherbench2/derived_variables.py:59-99 and 132-338 -- computed on the device
 from __future__ import annotations
 
 import dataclasses
+import math
 
 import numpy as np
 
 from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import derived_variables as dv
 from weatherbench2_b200 import xarray_lite as xl
 
@@ -30,7 +32,7 @@ class _WindVariable(dv.DerivedVariable):
 @dataclasses.dataclass
 class WindSpeed(_WindVariable):
   """Wind speed sqrt(u**2 + v**2) (derived_variables.py:77-99).  NumPy in ->
-  NumPy out; CUDA tensors in -> a CUDA tensor that the metric kernels read in
+  NumPy out; a CUDA tensor in -> a CUDA tensor that the metric kernels read in
   place."""
 
   @property
@@ -46,27 +48,10 @@ class WindSpeed(_WindVariable):
       if u.shape != v.shape:
         raise ValueError(f'{self.u_name} and {self.v_name} differ in shape')
     ctx = _lib.default_context()
-    ud, vd = u.data, v.data
-    if xl._is_torch(ud) and ud.is_cuda:  # pylint: disable=protected-access
-      import torch  # pylint: disable=import-outside-toplevel
-      a = ud.to(torch.float32).contiguous()
-      b = vd.to(torch.float32).contiguous().to(a.device)
-      out = torch.empty_like(a)
-      torch.cuda.current_stream(a.device).synchronize()
-      ctx.wind_speed(a.data_ptr(), b.data_ptr(), out.data_ptr(), a.numel())
-      ctx.synchronize()
-      data = out
-    else:
-      a = np.ascontiguousarray(np.asarray(u.values), dtype=np.float32)
-      b = np.ascontiguousarray(np.asarray(v.values), dtype=np.float32)
-      pa, pb = ctx.to_device(a), ctx.to_device(b)
-      po = ctx.malloc(max(a.nbytes, 4))
-      try:
-        ctx.wind_speed(pa, pb, po, a.size)
-        data = ctx.from_device(po, a.shape, np.float32)
-      finally:
-        for p in (pa, pb, po):
-          ctx.free(p)
+    n = math.prod(u.shape)
+    data, = _streamed.run_whole(
+        [u.data, v.data], [(u.shape, np.float32)],
+        lambda i, o: ctx.wind_speed(i[0], i[1], o[0], n), dtype=np.float32)
     coords = {k: c for k, c in u.coords.items()}
     result = xl.DataArray(data, u.dims, coords)
     if native:
@@ -81,6 +66,15 @@ GEOSTROPHIC_WIND_SPEED, U_GEOSTROPHIC, V_GEOSTROPHIC = 3, 4, 5
 AGEOSTROPHIC_WIND_SPEED, U_AGEOSTROPHIC, V_AGEOSTROPHIC = 6, 7, 8
 
 OMEGA = 7.292e-5  # radians / second (derived_variables.py:234)
+
+
+def check_same_grid(names, das):
+  """ValueError unless every variable of `das` (named `names`) has the first
+  one's dims, in any order, and sizes."""
+  for name, da in zip(names[1:], das[1:]):
+    if set(da.dims) != set(das[0].dims) or any(
+        da.sizes[d] != das[0].sizes[d] for d in das[0].dims):
+      raise ValueError(f'{names[0]!r} and {name!r} differ in dims or shape')
 
 
 def gradient_table(coord) -> tuple[np.ndarray, bool]:
@@ -115,7 +109,7 @@ def coriolis_parameter(latitude) -> np.ndarray:
 def wind_dynamics(dataset, kind: int, u_name=None, v_name=None, z_name=None):
   """One wb2_wind_dynamics call on the named variables of `dataset`.  The
   result keeps the first input's dims and coords; float32, on the device when
-  the inputs are CUDA tensors, else NumPy.  Float64 data is cast to float32 and
+  an input is a CUDA tensor, else NumPy.  Float64 data is cast to float32 and
   float32 coordinates are taken as float64 (DESIGN.md, "Wind dynamics")."""
   native = xl.is_native_xarray(dataset)
   ds = xl.from_xarray(dataset)
@@ -137,10 +131,7 @@ def wind_dynamics(dataset, kind: int, u_name=None, v_name=None, z_name=None):
   lead = (('level',) if vertical else ())
   outer = tuple(d for d in ref.dims if d not in spatial + lead)
   work = outer + lead + spatial
-  for da in das[1:]:
-    if set(da.dims) != set(ref.dims) or any(
-        da.sizes[d] != ref.sizes[d] for d in ref.dims):
-      raise ValueError(f'{names[0]} and {da.name} differ in dims or shape')
+  check_same_grid(names, das)
   lat = ref.coords['latitude'].values
   lon = ref.coords['longitude'].values
   lat_tab, lat_uniform = gradient_table(lat)
@@ -162,39 +153,10 @@ def wind_dynamics(dataset, kind: int, u_name=None, v_name=None, z_name=None):
     ctx.wind_dynamics(kind, by_name.get(u_name), by_name.get(v_name),
                       by_name.get(z_name), nouter, nlev, nlat, nlon, *strides,
                       lat_tab, lat_uniform, lon_tab, lon_uniform, cos_lat,
-                      coriolis, pressure, out)
+                      coriolis, pressure, out[0])
 
-  first = ref.data
-  if xl._is_torch(first) and first.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    xs = []
-    for da in das:
-      x = da.transpose(*work).data
-      if not xl._is_torch(x):  # pylint: disable=protected-access
-        x = torch.from_numpy(np.asarray(x))
-      xs.append(x.to(first.device, torch.float32).contiguous())
-    out = torch.empty(shape, device=first.device, dtype=torch.float32)
-    if out.numel():
-      torch.cuda.current_stream(first.device).synchronize()
-      call([x.data_ptr() for x in xs], out.data_ptr())
-      ctx.synchronize()
-    data = out
-  else:
-    xs = [np.ascontiguousarray(np.asarray(da.transpose(*work).values),
-                               dtype=np.float32) for da in das]
-    if not xs[0].size:
-      data = np.empty(shape, np.float32)
-    else:
-      ptrs, po = [], None
-      try:
-        for x in xs:
-          ptrs.append(ctx.to_device(x))
-        po = ctx.malloc(xs[0].nbytes)
-        call(ptrs, po)
-        data = ctx.from_device(po, shape, np.float32)
-      finally:
-        for p in ptrs + ([po] if po else []):
-          ctx.free(p)
+  data, = _streamed.run_whole([da.transpose(*work).data for da in das],
+                              [(shape, np.float32)], call, dtype=np.float32)
   coords = {k: c for k, c in ref.coords.items()}
   result = xl.DataArray(data, work, coords).transpose(*ref.dims)
   if xl._is_torch(result.data):  # pylint: disable=protected-access

@@ -443,6 +443,12 @@ class Staging:
     self.ptrs.append(ptr)
     return ptr
 
+  def malloc(self, nbytes: int) -> int:
+    """Uninitialised device buffer of `nbytes`."""
+    ptr = self.ctx.malloc(nbytes)
+    self.ptrs.append(ptr)
+    return ptr
+
   def upload(self, op: Operand) -> Operand:
     """`op` re-addressed on the device: the smallest contiguous span of its
     backing array (same strides), or, for a gathered operand, only the slabs it

@@ -1,12 +1,17 @@
-"""Where the data of a streamed operator lives decides which C entry runs it.
+"""Where an operator's data lives decides how its C entry runs: the one
+residency rule of the operators, in two forms.
 
 The quantile, average, time-window, precipitation-accumulation and
 climatology operators each have an entry pair in `_lib.Context`:
 `X(x, dtype, *args, *outputs)` reads device addresses, and
 `X_host(x, dtype, *args, budget, *outputs)` streams host memory through the
 device in bands whose device footprint stays within `budget` bytes.  `run`
-holds the one rule that picks between them, so each operator only computes
-its layout."""
+holds the rule that picks between them.
+
+The derived-variable, ensemble-mean, spectrum-interpolation and staged regrid
+operators have only the device entry.  `run_whole` runs it on CUDA operands
+in place, and otherwise uploads the host operands whole and copies the results
+back.  Either way each operator only computes its layout."""
 from __future__ import annotations
 
 import functools
@@ -16,6 +21,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _spatial
 from weatherbench2_b200 import xarray_lite as xl
 
 
@@ -69,3 +75,54 @@ def run(entry: str, data, args: Sequence, outputs: Sequence, budget: int, *,
     fn(ptr(x), code, *args, *extra,
        *[None if a is None else ptr(a) for a in res], **kwargs)
   return res
+
+
+def run_whole(datas: Sequence, outputs: Sequence, call, *,
+              perms: Optional[Sequence] = None, dtype=None) -> list:
+  """Runs `call(in_ptrs, out_ptrs)` once on device copies of `datas` (the
+  operands' `.data`) and returns its outputs in order.
+
+  When any operand is a CUDA tensor the call runs on that tensor's device:
+  every operand is moved there (NumPy through `torch.from_numpy`), permuted by
+  its entry of `perms`, cast to `dtype` and made contiguous, and the outputs
+  are `torch.empty` on that device.  Otherwise every operand is read as NumPy,
+  transposed and made contiguous in `dtype`, uploaded whole, and the outputs
+  come back as NumPy; every device buffer is freed when the call returns or
+  raises.  `perms` None, or a None entry, keeps the stored order, and `dtype`
+  None the stored dtype.  `outputs` lists one (shape, NumPy dtype) per output.
+  When every output is empty, `call` is not made and nothing is uploaded."""
+  perms = [None] * len(datas) if perms is None else perms
+  empty = not any(math.prod(shape) for shape, _ in outputs)
+  device = next((x.device for x in datas
+                 if xl._is_torch(x) and x.is_cuda), None)  # pylint: disable=protected-access
+  if device is not None:
+    import torch  # pylint: disable=import-outside-toplevel
+    res = [torch.empty(shape, dtype=_torch_dtype(dt), device=device)
+           for shape, dt in outputs]
+    if empty:
+      return res
+    xs = []
+    for x, perm in zip(datas, perms):
+      if not xl._is_torch(x):  # pylint: disable=protected-access
+        x = torch.from_numpy(xl._np(x))  # pylint: disable=protected-access
+      if perm is not None:
+        x = x.permute(*perm)
+      xs.append(x.to(device, None if dtype is None else _torch_dtype(dtype))
+                .contiguous())
+    # No host wait: _LockedLib orders the entry after torch's current stream
+    # and that stream after the entry, so torch may reuse `xs` once freed.
+    call([x.data_ptr() for x in xs], [r.data_ptr() for r in res])
+    return res
+  if empty:
+    return [np.empty(shape, dt) for shape, dt in outputs]
+  xs = [np.ascontiguousarray(
+      xl._np(x) if perm is None else np.transpose(xl._np(x), perm),  # pylint: disable=protected-access
+      dtype=dtype) for x, perm in zip(datas, perms)]
+  ctx = _lib.default_context()
+  with _spatial.Staging(ctx) as stage:
+    ins = [stage.array(x) for x in xs]
+    outs = [stage.malloc(math.prod(shape) * np.dtype(dt).itemsize)
+            for shape, dt in outputs]
+    call(ins, outs)
+    return [ctx.from_device(p, shape, dt)
+            for p, (shape, dt) in zip(outs, outputs)]

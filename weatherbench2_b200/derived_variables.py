@@ -21,6 +21,7 @@ import typing as t
 import numpy as np
 
 from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import xarray_lite as xl
 
 EARTH_RADIUS_M = 1000 * (6357 + 6378) / 2  # weatherbench2/schema.py:59
@@ -122,10 +123,8 @@ class ZonalEnergySpectrum(DerivedVariable):
       import torch  # pylint: disable=import-outside-toplevel
       x = data.to(torch.float32).contiguous()
       out = torch.zeros(res_shape, device=data.device, dtype=torch.float32)
-      torch.cuda.current_stream(data.device).synchronize()
       ctx.zonal_spectrum(x.data_ptr(), nfield, nlat, nlon, scale,
                          out.data_ptr(), time_sum_dim is not None, nout)
-      ctx.synchronize()
       values = out
     else:
       # host data: streamed through double-buffered staging; with a time sum
@@ -261,23 +260,11 @@ def interpolate_spectral_frequencies(spectrum, wavenumber_dim: str,
   nfield = int(np.prod(oshape)) if oshape else 1
   nf = frequencies.size
   ctx = _lib.default_context()
-  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    x = data.to(torch.float32).contiguous()
-    out = torch.empty(oshape + (nlat, nf), device=x.device, dtype=torch.float32)
-    ctx.spectrum_interp(x.data_ptr(), nfield, nlat, nk, table, frequencies,
-                        out.data_ptr())
-    values = out
-  else:
-    x = np.ascontiguousarray(np.asarray(data), dtype=np.float32)
-    src = ctx.to_device(x)
-    dst = ctx.malloc(max(4, nfield * nlat * nf * 4))
-    try:
-      ctx.spectrum_interp(src, nfield, nlat, nk, table, frequencies, dst)
-      values = ctx.from_device(dst, oshape + (nlat, nf), np.float32)
-    finally:
-      ctx.free(src)
-      ctx.free(dst)
+  values, = _streamed.run_whole(
+      [data], [(oshape + (nlat, nf), np.float32)],
+      lambda i, o: ctx.spectrum_interp(i[0], nfield, nlat, nk, table,
+                                       frequencies, o[0]),
+      dtype=np.float32)
   dims = outer + ('latitude', 'frequency')
   coords = {k: c for k, c in work.coords.items()
             if wavenumber_dim not in c.dims and k not in ('frequency',

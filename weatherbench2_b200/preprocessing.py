@@ -55,22 +55,10 @@ def compute_ensemble_mean(dataset, realization_name: str = REALIZATION,
     off = np.zeros(1, dtype=np.int64)
     coords = {k: c for k, c in work.coords.items()
               if realization_name not in c.dims}
-    if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-      import torch  # pylint: disable=import-outside-toplevel
-      x = data.to(torch.float32).contiguous()
-      res = torch.empty(shape, device=x.device, dtype=torch.float32)
-      ctx.ens_mean(x.data_ptr(), m, cells, off, slab, skipna, res.data_ptr())
-      values = res
-    else:
-      x = np.ascontiguousarray(np.asarray(data), dtype=np.float32)
-      src = ctx.to_device(x)
-      dst = ctx.malloc(max(4, cells * 4))
-      try:
-        ctx.ens_mean(src, m, cells, off, slab, skipna, dst)
-        values = ctx.from_device(dst, shape, np.float32)
-      finally:
-        ctx.free(src)
-        ctx.free(dst)
+    values, = _streamed.run_whole(
+        [data], [(shape, np.float32)],
+        lambda i, o: ctx.ens_mean(i[0], m, cells, off, slab, skipna, o[0]),
+        dtype=np.float32)
     out[name] = xl.DataArray(values, dims, coords, name, v.attrs)
   return xl.to_xarray(out) if native else out
 

@@ -19,6 +19,7 @@ from typing import Optional
 import numpy as np
 
 from weatherbench2_b200 import _lib
+from weatherbench2_b200 import _streamed
 from weatherbench2_b200 import xarray_lite as xl
 
 _DT = np.float32
@@ -242,29 +243,17 @@ class Regridder:
     batch = shape[:-2]
     nfield = int(np.prod(batch)) if batch else 1
     tshape = batch + self.target.shape
-    if is_torch and field.is_cuda:
-      import torch  # pylint: disable=import-outside-toplevel
-      x = field.to(torch.float32).contiguous()
-      out = torch.empty(tshape, device=field.device, dtype=torch.float32)
-      stream = torch.cuda.current_stream(field.device)
-      stream.synchronize()
-      self.regrid_device(ctx, x.data_ptr(), out.data_ptr(), nfield)
-      ctx.synchronize()
-      return out
-    x = np.ascontiguousarray(np.asarray(field), dtype=np.float32)
-    nt = self.target.shape[0] * self.target.shape[1]
-    out = ctx.pinned_result(tshape, np.float32)
-    if nfield and self.regrid_host(ctx, x.ctypes.data, out.ctypes.data,
-                                   nfield):
-      return out  # streamed: H2D, kernel and D2H of neighbouring groups overlap
-    src = ctx.to_device(x)
-    dst = ctx.malloc(max(1, nfield * nt * 4))
-    try:
-      self.regrid_device(ctx, src, dst, nfield)
-      return ctx.from_device(dst, tshape, np.float32)
-    finally:
-      ctx.free(src)
-      ctx.free(dst)
+    x = field
+    if not (is_torch and field.is_cuda):
+      x = np.ascontiguousarray(np.asarray(field), dtype=np.float32)
+      out = ctx.pinned_result(tshape, np.float32)
+      if nfield and self.regrid_host(ctx, x.ctypes.data, out.ctypes.data,
+                                     nfield):
+        return out  # streamed: H2D, kernel and D2H of neighbouring groups overlap
+    return _streamed.run_whole(
+        [x], [(tshape, np.float32)],
+        lambda i, o: self.regrid_device(ctx, i[0], o[0], nfield),
+        dtype=np.float32)[0]
 
   def regrid_host(self, ctx: _lib.Context, src_ptr: int, dst_ptr: int,
                   nfield: int) -> bool:
