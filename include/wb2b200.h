@@ -815,15 +815,22 @@ int wb2_gaussian_metrics(wb2_ctx* ctx, const void* mean, const void* std,
  * Input slabs are (lon_src, lat_src) with lat contiguous, output slabs
  * (lon_tgt, lat_tgt) float32, exactly the reference's layout (regridding.py:190).
  * A NaN weight row (target cell not covered, regridding.py:367-371) is flagged
- * by a negative tap count and yields NaN.
+ * by nan_row and yields NaN; a row without taps that is not flagged gives
+ * 0 / 0 = NaN.
+ * Banded semantics: a target cell sees only its own stored taps, NaN inputs
+ * are missing, and +-inf propagate in IEEE arithmetic (+inf and -inf in one
+ * footprint give NaN).  The reference contracts with the dense matrices, where
+ * 0 * inf turns the whole 2-D slice NaN; here only the cells whose footprint
+ * holds the infinity are affected, whichever kernel runs.
  */
 typedef struct {
   int32_t n_src;            /* source axis length                              */
   int32_t n_tgt;            /* target axis length                              */
-  const int32_t* row_ptr;   /* host [n_tgt + 1] CSR offsets; row_ptr[i+1] <
-                               row_ptr[i] never happens; uncovered rows have
-                               zero taps and nan_row[i] = 1                    */
-  const int32_t* col_idx;   /* host [nnz] source indices                       */
+  const int32_t* row_ptr;   /* host [n_tgt + 1] CSR offsets, row_ptr[0] = 0,
+                               non-decreasing; uncovered rows have zero taps
+                               and nan_row[i] = 1                              */
+  const int32_t* col_idx;   /* host [nnz] source indices, strictly increasing
+                               within each row (rejected otherwise)            */
   const float* val;         /* host [nnz] weights (rows sum to 1)              */
   const uint8_t* nan_row;   /* host [n_tgt] 1 = output NaN                     */
 } wb2_csr;

@@ -17,6 +17,7 @@ import contextlib
 import ctypes as C
 
 import numpy as np
+import scipy.sparse
 
 from weatherbench2_b200 import _lib
 
@@ -435,19 +436,19 @@ class FakeContext:
 
   # -- K5 / K8: regridding -----------------------------------------------------------
   @staticmethod
-  def _dense(csr: _lib.CsrSpec) -> np.ndarray:
-    w = np.zeros((csr.n_tgt, csr.n_src))
-    for i in range(csr.n_tgt):
-      lo, hi = csr.row_ptr[i], csr.row_ptr[i + 1]
-      w[i, csr.col_idx[lo:hi]] = csr.val[lo:hi]
-      if csr.nan_row[i]:
-        w[i] = np.nan
-    return w
+  def _sparse(csr: _lib.CsrSpec):
+    nnz = int(csr.row_ptr[csr.n_tgt])
+    return scipy.sparse.csr_matrix(
+        (csr.val[:nnz].astype(np.float64), csr.col_idx[:nnz],
+         csr.row_ptr[:csr.n_tgt + 1]), shape=(csr.n_tgt, csr.n_src))
 
   def regrid_conservative(self, src, dst, nfield, src_stride, dst_stride, lon_w,
                           lat_w):
+    # Banded like the kernels: only stored taps contribute, so an infinity
+    # reaches only the cells whose footprint holds it (a dense contraction
+    # would multiply it by the zero weights and spread NaN).
     self.calls.append(('regrid_conservative', int(nfield)))
-    wlon, wlat = self._dense(lon_w), self._dense(lat_w)
+    wlon, wlat = self._sparse(lon_w), self._sparse(lat_w)
     ns = lon_w.n_src * lat_w.n_src
     nt = lon_w.n_tgt * lat_w.n_tgt
     for i in range(nfield):
@@ -455,9 +456,11 @@ class FakeContext:
           lon_w.n_src, lat_w.n_src).astype(np.float64)
       ok = ~np.isnan(x)
       with np.errstate(invalid='ignore', divide='ignore'):
-        num = np.einsum('ab,cd,bd->ac', wlon, wlat, np.where(ok, x, 0.0))
-        den = np.einsum('ab,cd,bd->ac', wlon, wlat, ok.astype(np.float64))
+        num = (wlat @ (wlon @ np.where(ok, x, 0.0)).T).T
+        den = (wlat @ (wlon @ ok.astype(np.float64)).T).T
         res = num / den
+        res[lon_w.nan_row.astype(bool), :] = np.nan
+        res[:, lat_w.nan_row.astype(bool)] = np.nan
       _view(dst + i * dst_stride * 4, nt, np.float32)[...] = res.astype(
           np.float32).reshape(-1)
 

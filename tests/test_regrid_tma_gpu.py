@@ -65,11 +65,10 @@ def test_tma_path_equals_ldg_path_and_oracle(monkeypatch, nls, nlas, nlt, nlat):
   np.testing.assert_array_equal(res['tma'], res['ldg'])
   want = orc.conservative_regrid(
       x, orc.Grid(slon, slat, includes_poles=True),
-      orc.Grid(tlon, tlat, includes_poles=bool(nlat % 2)))
+      orc.Grid(tlon, tlat, includes_poles=True))
   got = res['tma'].reshape(nfield, nlt, nlat)
-  if nlat % 2:
-    np.testing.assert_array_equal(np.isnan(got), np.isnan(want))
-    np.testing.assert_allclose(got, want, rtol=1e-5, atol=2e-6)
+  np.testing.assert_array_equal(np.isnan(got), np.isnan(want))
+  np.testing.assert_allclose(got, want, rtol=1e-5, atol=2e-6)
 
 
 def test_padded_field_strides_and_unaligned_base(monkeypatch):

@@ -21,6 +21,9 @@
 // Arithmetic is float32 like the reference (JAX default); the order of
 // summation differs (taps in ascending source index).  Target cells the source
 // grid does not cover (NaN weight rows, regridding.py:367-371, 493-497) are NaN.
+// Banded semantics: a target cell sees only its own taps, so +-inf reach only
+// the cells whose footprint holds them (the reference's dense contraction
+// multiplies them by zero weights and turns the whole slice NaN).
 //
 // Roofline: HBM, 4 B read per source cell + 4 B written per target cell.
 #include <algorithm>
@@ -40,6 +43,9 @@ struct RegridParams {
   const int32_t* grp_rows;  // [ngroups][maxnb] source rows of the group (-1 pad)
   const float* grp_w;       // [ngroups][maxnb][kRgGroup]
   const int32_t* grp_nb;    // [ngroups]
+  const int32_t* lon_ptr;   // [nlon_t + 1] the longitude CSR, for the columns
+  const int32_t* lon_idx;   //   that hold a NaN or an infinity
+  const float* lon_val;
   const uint8_t* lon_nan;   // [nlon_t]
   const int32_t* lat_ptr;   // [nlat_t + 1]
   const int32_t* lat_idx;
@@ -48,6 +54,28 @@ struct RegridParams {
   int32_t nlon_s, nlat_s, nlon_t, nlat_t;
   int32_t ngroups, maxnb;
 };
+
+// Column d of a group whose accumulation met a NaN or an infinity: y and v of
+// each target over its OWN taps, in CSR order, NaN as missing (out of line, so
+// that the hot loop keeps its registers).
+__device__ __noinline__ void regrid_own_taps(const float* __restrict__ x, int d, int nlat_s,
+                                             const int32_t* __restrict__ ptr, int na,
+                                             const int32_t* __restrict__ idx,
+                                             const float* __restrict__ val, float* ybuf) {
+  for (int a = 0; a < na; ++a) {
+    float yy = 0.f, vv = 0.f;
+    const int t1 = __ldg(ptr + a + 1);
+    for (int tp = __ldg(ptr + a); tp < t1; ++tp) {
+      const float w = __ldg(val + tp);
+      const float xq = __ldg(x + int64_t(__ldg(idx + tp)) * nlat_s + d);
+      const bool ok = xq == xq;
+      yy = fmaf(w, ok ? xq : 0.f, yy);
+      vv = fmaf(w, ok ? 1.f : 0.f, vv);
+    }
+    ybuf[(a * 2 + 0) * nlat_s + d] = yy;
+    ybuf[(a * 2 + 1) * nlat_s + d] = vv;
+  }
+}
 
 template <int kRgDpt>
 __global__ void __launch_bounds__(kRgThreads) regrid_kernel(const RegridParams p) {
@@ -78,14 +106,16 @@ __global__ void __launch_bounds__(kRgThreads) regrid_kernel(const RegridParams p
 
   // ---- stage 1: contract over source longitude, every source row read once ---
   // The valid-weight sum v = sum_b W[a,b] [x[b,d] not NaN] equals the plain row
-  // sum of the weights unless a NaN is met, so the hot loop only accumulates y
-  // and remembers whether its column saw a NaN; columns that did recompute v
-  // exactly (second pass over the same rows, served by L1/L2).
-  float y[kRgDpt][kRgGroup], v[kRgDpt][kRgGroup];
-  bool saw_nan[kRgDpt];
+  // sum of the weights unless a NaN is met, so the hot loop only accumulates
+  // y = sum_b W[a,b] x[b,d] WITHOUT looking at the values: a NaN or an infinity
+  // anywhere in the column makes some y of the group NaN or infinite (the dense
+  // table's zeros give 0 * inf = NaN).  Those columns recompute y and v over
+  // each target's OWN taps (second pass over the same rows, served by L1/L2),
+  // so a target sees only its own taps, exactly as in regrid_tma_kernel.
+  const float infv = __int_as_float(0x7f800000);
+  float y[kRgDpt][kRgGroup];
 #pragma unroll
   for (int i = 0; i < kRgDpt; ++i) {
-    saw_nan[i] = false;
 #pragma unroll
     for (int a = 0; a < kRgGroup; ++a) y[i][a] = 0.f;
   }
@@ -102,45 +132,28 @@ __global__ void __launch_bounds__(kRgThreads) regrid_kernel(const RegridParams p
     const float4 w4 = *reinterpret_cast<const float4*>(wtab + bi * kRgGroup);
     const float w[kRgGroup] = {w4.x, w4.y, w4.z, w4.w};
 #pragma unroll
-    for (int i = 0; i < kRgDpt; ++i) {
-      const bool ok = xv[i] == xv[i];
-      saw_nan[i] |= !ok;
-      const float x0 = ok ? xv[i] : 0.f;
+    for (int i = 0; i < kRgDpt; ++i)
 #pragma unroll
-      for (int a = 0; a < kRgGroup; ++a) y[i][a] = fmaf(w[a], x0, y[i][a]);
-    }
+      for (int a = 0; a < kRgGroup; ++a) y[i][a] = fmaf(w[a], xv[i], y[i][a]);
   }
-  // v for NaN-free columns: the weights' row sums, added in the same order and
+  // v for finite columns: the weights' row sums, added in the same order and
   // rounding as the explicit accumulation would (bit-identical)
   float wsum[kRgGroup];
 #pragma unroll
   for (int a = 0; a < kRgGroup; ++a) wsum[a] = s_wsum[a];
 #pragma unroll
   for (int i = 0; i < kRgDpt; ++i) {
-#pragma unroll
-    for (int a = 0; a < kRgGroup; ++a) v[i][a] = wsum[a];
-    if (saw_nan[i]) {
-      const int d = threadIdx.x + i * kRgThreads;
-#pragma unroll
-      for (int a = 0; a < kRgGroup; ++a) v[i][a] = 0.f;
-      for (int bi = 0; bi < nb; ++bi) {
-        const float xv = __ldg(x + int64_t(rows[bi]) * p.nlat_s + d);
-        const float one = xv == xv ? 1.f : 0.f;
-#pragma unroll
-        for (int a = 0; a < kRgGroup; ++a)
-          v[i][a] = fmaf(wtab[bi * kRgGroup + a], one, v[i][a]);
-      }
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < kRgDpt; ++i) {
     const int d = threadIdx.x + i * kRgThreads;
     if (d < p.nlat_s) {
+      bool bad = false;
 #pragma unroll
       for (int a = 0; a < kRgGroup; ++a) {
+        bad |= !(fabsf(y[i][a]) < infv);
         ybuf[(a * 2 + 0) * p.nlat_s + d] = y[i][a];
-        ybuf[(a * 2 + 1) * p.nlat_s + d] = v[i][a];
+        ybuf[(a * 2 + 1) * p.nlat_s + d] = wsum[a];
       }
+      if (bad)
+        regrid_own_taps(x, d, p.nlat_s, p.lon_ptr + a0, na, p.lon_idx, p.lon_val, ybuf);
     }
   }
   __syncthreads();
@@ -182,6 +195,13 @@ static int check_csr(const wb2_csr* m, const char* name) {
   for (int i = 0; i < nnz; ++i)
     WB2_REQUIRE(m->col_idx[i] >= 0 && m->col_idx[i] < m->n_src, "%s: col_idx out of range",
                 name);
+  // Both kernels add a target's taps in ascending source order; the TMA kernel
+  // walks the CSR as given and this one the sorted union of a group's rows, so
+  // they agree only when every row is sorted and free of duplicates.
+  for (int i = 0; i < m->n_tgt; ++i)
+    for (int tp = m->row_ptr[i] + 1; tp < m->row_ptr[i + 1]; ++tp)
+      WB2_REQUIRE(m->col_idx[tp] > m->col_idx[tp - 1],
+                  "%s: col_idx must be strictly increasing within a row (row %d)", name, i);
   return WB2_OK;
 }
 
@@ -245,16 +265,19 @@ extern "C" int wb2_regrid_conservative(wb2_ctx* ctx, const float* src, float* ds
     for (int a = g * kRgGroup; a < std::min(nlon_t, (g + 1) * kRgGroup); ++a)
       for (int tp = lon_w->row_ptr[a]; tp < lon_w->row_ptr[a + 1]; ++tp) {
         const size_t bi = std::lower_bound(r.begin(), r.end(), lon_w->col_idx[tp]) - r.begin();
-        // duplicate taps (never produced by the reference's formulas) add up
-        h_w[(size_t(g) * maxnb + bi) * kRgGroup + (a - g * kRgGroup)] += lon_w->val[tp];
+        h_w[(size_t(g) * maxnb + bi) * kRgGroup + (a - g * kRgGroup)] = lon_w->val[tp];
       }
   }
 
   const int nlat_nnz = lat_w->row_ptr[lat_w->n_tgt] > 0 ? lat_w->row_ptr[lat_w->n_tgt] : 1;
+  const int nlon_nnz = std::max(1, lon_w->row_ptr[nlon_t]);
   Packer pk(ctx);
   size_t o1 = pk.add(h_rows.data(), h_rows.size() * 4);
   size_t o2 = pk.add(h_w.data(), h_w.size() * 4);
   size_t o3 = pk.add(h_nb.data(), h_nb.size() * 4);
+  size_t o9 = pk.add(lon_w->row_ptr, size_t(nlon_t + 1) * 4);
+  size_t o10 = pk.add(lon_w->col_idx, size_t(nlon_nnz) * 4);
+  size_t o11 = pk.add(lon_w->val, size_t(nlon_nnz) * 4);
   size_t o4 = pk.add(lon_w->nan_row, size_t(lon_w->n_tgt));
   size_t o5 = pk.add(lat_w->row_ptr, size_t(lat_w->n_tgt + 1) * 4);
   size_t o6 = pk.add(lat_w->col_idx, size_t(nlat_nnz) * 4);
@@ -267,6 +290,8 @@ extern "C" int wb2_regrid_conservative(wb2_ctx* ctx, const float* src, float* ds
   p.src_field_stride = src_field_stride; p.dst_field_stride = dst_field_stride;
   p.grp_rows = pk.dev<int32_t>(o1); p.grp_w = pk.dev<float>(o2);
   p.grp_nb = pk.dev<int32_t>(o3); p.lon_nan = pk.dev<uint8_t>(o4);
+  p.lon_ptr = pk.dev<int32_t>(o9); p.lon_idx = pk.dev<int32_t>(o10);
+  p.lon_val = pk.dev<float>(o11);
   p.lat_ptr = pk.dev<int32_t>(o5); p.lat_idx = pk.dev<int32_t>(o6);
   p.lat_val = pk.dev<float>(o7); p.lat_nan = pk.dev<uint8_t>(o8);
   p.nlon_s = lon_w->n_src; p.nlat_s = lat_w->n_src;
