@@ -17,6 +17,7 @@ headline contract line is bench.py.
   python benchmarks/bench_kernels.py --kernel column_integral --steps 20
   python benchmarks/bench_kernels.py --kernel quantile --steps 5
   python benchmarks/bench_kernels.py --kernel average --steps 5
+  python benchmarks/bench_kernels.py --kernel slab_gather --steps 10
 """
 import argparse
 import json
@@ -994,6 +995,134 @@ def bench_average(args):
       h2d_pageable_GBps=h2d, frac_of_h2d=gbs / h2d)), flush=True)
 
 
+def bench_slab_gather(args):
+  """wb2_slab_gather (the copy of weatherbench2_b200.reindexing) against the
+  same gather in torch (index_select, masked_fill with NaN, .to(float32)),
+  on both of its kernels: probabilistic forecasts (10 members x 61 leads x 28
+  inits) from 4 years of 6-hourly 13x121x240 truth and a 0.25-degree 13-level
+  forecast on valid time (slabs of 377,520 and 13.5 M elements: the chunked
+  16-byte kernel), and 64x32 single-level forecasts (slabs of 2048: the flat
+  kernel).  Bytes are the output written plus, per output slab, its source
+  slab read.  Then a memmap truth through the host entry: bytes moved and rate."""
+  import tempfile
+  import time
+  import pandas as pd
+  torch, _lib, ctx = setup()
+  from weatherbench2_b200 import reindexing as ri
+  card = _card()
+  rng = np.random.default_rng(0)
+
+  def prob_offsets(ntime_truth, members, leads, inits):
+    truth = pd.date_range('1990-01-01', periods=ntime_truth, freq='6h')
+    out_t = pd.date_range('1992-01-01', periods=inits, freq='6h')
+    sampled = ri.get_sampled_init_times(
+        out_t, climatology_start_year=1990, climatology_end_year=1992,
+        ensemble_size=members, seed=1)
+    deltas = np.arange(leads) * np.timedelta64(6, 'h')
+    need = sampled[:, None, :] + deltas[None, :, None]
+    return truth.get_indexer(need.reshape(-1)).astype(np.int64)
+
+  def run_case(name, src, pos, slab, out_dtype):
+    """pos: source slab per output slab, -1 for NaN."""
+    to = torch.float32 if out_dtype == _lib.F32 else torch.float64
+    out = torch.empty((pos.size, slab), dtype=to, device='cuda')
+    code = _lib.F32 if src.dtype == torch.float32 else _lib.F64
+    offsets = np.where(pos < 0, -1, pos * slab)
+    dev = lambda: ctx.slab_gather(src.data_ptr(), code, src.numel(), slab,
+                                  pos.size, offsets, out.data_ptr(), out_dtype)
+    src2 = src.view(-1, slab)
+    idx = torch.from_numpy(np.maximum(pos, 0)).cuda()
+    miss = torch.from_numpy(pos < 0).cuda()[:, None]
+    base = lambda: src2.index_select(0, idx).masked_fill_(miss, float('nan')).to(to)
+    dev()
+    ref = base()
+    torch.cuda.synchronize()
+    for r in range(0, pos.size, 256):  # equal, NaN where NaN (in row blocks)
+      a, b = out[r:r + 256], ref[r:r + 256]
+      assert torch.equal(a.isnan(), b.isnan()) and torch.equal(
+          torch.nan_to_num(a), torch.nan_to_num(b)), name
+    del ref, a, b
+    # every output slab written once and its source slab read once (a
+    # source slab used by several outputs is read again unless L2 holds it)
+    nread = int((pos >= 0).sum()) * slab * src.element_size()
+    nbytes = out.numel() * out.element_size() + nread
+    for label, fn in (('wb2_slab_gather', dev), ('torch baseline', base)):
+      ms = timeit(fn, args.steps)
+      report(f'slab_gather {name} [{label}]', ms, nbytes, pos.size, 'slabs',
+             card)
+    del out
+    torch.cuda.empty_cache()
+
+  ncell = 13 * 121 * 240
+  ntruth = 4 * 1461
+  truth = torch.empty((ntruth, ncell), dtype=torch.float32, device='cuda')
+  truth.normal_()
+  run_case('prob 10x61x28 from 4y 6-hourly 13x121x240 f32', truth,
+           prob_offsets(ntruth, 10, 61, 28), ncell, _lib.F32)
+  del truth
+  torch.cuda.empty_cache()
+  # forecast on valid time: 8 inits 12 h apart, 5 leads 6 h apart, valid_and_delta
+  init = np.arange(8) * 12
+  leads = np.arange(5) * 6
+  kept = np.arange(0, 5, 2)
+  times = np.unique(init[:, None] + leads[kept][None, :])
+  ii = pd.Index(init).get_indexer((times[:, None] - leads[kept][None, :]).reshape(-1))
+  pos = np.where(ii < 0, -1, ii * 5 + np.tile(kept, times.size))
+  slab = 13 * NLAT * NLON
+  for dt, tag in ((torch.float32, 'f32'), (torch.float64, 'f64')):
+    fc = torch.empty((8 * 5, slab), dtype=dt, device='cuda')
+    fc.normal_()
+    run_case(f'valid time 13x721x1440 {tag}->f32 ({pos.size} slabs)', fc, pos,
+             slab, _lib.F32)
+    del fc
+    torch.cuda.empty_cache()
+  small = torch.empty((ntruth, 64 * 32), dtype=torch.float32, device='cuda')
+  small.normal_()
+  run_case('prob 10x61x280 from 4y 6-hourly 64x32 f32 (flat kernel)', small,
+           prob_offsets(ntruth, 10, 61, 280), 64 * 32, _lib.F32)
+  del small
+  torch.cuda.empty_cache()
+
+  # host entry: one year of 13x121x240 truth on a memmap, 10 x 61 x 4 slabs
+  with tempfile.TemporaryDirectory() as tmp:
+    nt = 1464
+    mm = np.memmap(os.path.join(tmp, 'truth.f32'), np.float32, 'w+',
+                   shape=(nt, ncell))
+    block = rng.standard_normal((61, ncell), dtype=np.float32)
+    for i in range(0, nt, 61):
+      mm[i:i + 61] = block[:nt - i]
+    mm.flush()
+    pos = prob_offsets(ntruth, 10, 61, 4) % nt
+    offsets = np.where(pos < 0, -1, pos * ncell)
+    out = ctx.pinned_result((pos.size, ncell), np.float32)
+    run = lambda: ctx.slab_gather_host(
+        mm.ctypes.data, _lib.F32, mm.size, ncell, pos.size, offsets,
+        ri.STREAM_BUDGET_BYTES, out.ctypes.data, _lib.F32)
+    run()
+    ctx.reset_transfer_stats()
+    t0 = time.perf_counter()
+    for _ in range(args.steps):
+      run()
+    s = (time.perf_counter() - t0) / args.steps
+    st = ctx.transfer_stats()
+    moved = (st['h2d_bytes'] + st['d2h_bytes']) / args.steps
+    probe = np.asarray(mm[:256]).reshape(-1)
+    dev = torch.empty(probe.size, device='cuda', dtype=torch.float32)
+    dev.copy_(torch.from_numpy(probe))
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(3):
+      dev.copy_(torch.from_numpy(probe))
+    torch.cuda.synchronize()
+    h2d = 3 * probe.nbytes / (time.perf_counter() - t0) / 1e9
+    print(json.dumps(dict(
+        card, kernel='slab_gather host memmap 1y 13x121x240 -> 10x61x4 slabs',
+        ms=s * 1e3, h2d_GB=st['h2d_bytes'] / args.steps / 1e9,
+        d2h_GB=st['d2h_bytes'] / args.steps / 1e9,
+        moved_GBps=moved / s / 1e9, h2d_pageable_GBps=h2d)), flush=True)
+    del mm
+
+
 if __name__ == '__main__':
   ap = argparse.ArgumentParser()
   ap.add_argument('--kernel', required=True,
@@ -1002,7 +1131,7 @@ if __name__ == '__main__':
                            'climatology_quantile', 'resample',
                            'wind_dynamics', 'precip_accumulation',
                            'column_integral', 'thermo', 'quantile',
-                           'average'])
+                           'average', 'slab_gather'])
   ap.add_argument('--steps', type=int, default=10)
   ap.add_argument('--fields', type=int, default=39)
   ap.add_argument('--members', type=int, nargs='+', default=[50])
@@ -1018,4 +1147,5 @@ if __name__ == '__main__':
    'column_integral': bench_column_integral,
    'thermo': bench_thermo,
    'quantile': bench_quantile,
-   'average': bench_average}[a.kernel](a)
+   'average': bench_average,
+   'slab_gather': bench_slab_gather}[a.kernel](a)

@@ -921,6 +921,35 @@ int wb2_zonal_spectrum_latsum_host(wb2_ctx* ctx, const float* x, int64_t nfield,
                                    const double* scale, float* out_host,
                                    int64_t nfield_out);
 
+/* ---- slab gather: reindexing in time --------------------------------------------
+ * wb2_slab_gather is the copy of weatherbench2_b200/reindexing.py (the
+ * reference's expand_climatology.py, index_on_valid_time.py and
+ * compute_probabilistic_climatological_forecasts.py):
+ *   out[s][i] = offsets[s] < 0 ? NaN : (out_dtype) src[offsets[s] + i],
+ *   0 <= s < nslab, 0 <= i < slab
+ * src        device array of src_dtype (WB2_F32 / WB2_F64) of src_elems elements
+ * offsets    host [nslab]; a negative entry fills its slab with NaN, any other
+ *            must satisfy offsets[s] + slab <= src_elems.  The whole table is
+ *            checked before anything is launched.
+ * out        device [nslab][slab] of out_dtype (WB2_F32 / WB2_F64); float64 to
+ *            float32 rounds to nearest (NumPy's astype), so the result is exact.
+ * slab == 0 or nslab == 0 launches nothing.  Slabs of 4096 elements or more are
+ * copied by CTAs of 4096 elements with 16-byte accesses where source and output
+ * alignment allow; shorter slabs by CTAs over the flattened output.            */
+int wb2_slab_gather(wb2_ctx* ctx, const void* src, int src_dtype, int64_t src_elems,
+                    int64_t slab, int64_t nslab, const int64_t* offsets, void* out,
+                    int out_dtype);
+
+/* wb2_slab_gather on a HOST source (NumPy / memmap) into a HOST out, in bands of
+ * consecutive output slabs, double buffered.  Each band uploads every distinct
+ * source range it references once (ranges that touch or overlap are one copy),
+ * so a source slab no output references is never read; a slab that does not fit
+ * is split into pieces.  `budget` bounds the device bytes of the two staging
+ * buffers; it must hold at least one element in each.                          */
+int wb2_slab_gather_host(wb2_ctx* ctx, const void* src, int src_dtype, int64_t src_elems,
+                         int64_t slab, int64_t nslab, const int64_t* offsets, size_t budget,
+                         void* out, int out_dtype);
+
 #ifdef __cplusplus
 }
 #endif

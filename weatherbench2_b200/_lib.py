@@ -224,6 +224,11 @@ PROTOTYPES = {
         _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
         C.c_int64, C.POINTER(C.c_double), C.c_int64, C.c_int64, C.c_int,
         C.c_size_t, _P, _P, _P]),
+    'wb2_slab_gather': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, _I64P, _P, C.c_int]),
+    'wb2_slab_gather_host': (C.c_int, [
+        _P, _P, C.c_int, C.c_int64, C.c_int64, C.c_int64, _I64P, C.c_size_t, _P,
+        C.c_int]),
 }
 # wb2_average: samples per chunk of the fixed summation order
 AVERAGE_CHUNK = 65536
@@ -899,6 +904,27 @@ class Context:
         int(bool(skipna)), int(budget), _P(mean) if mean else None,
         _P(mean_sq) if mean_sq else None, _P(frac) if frac else None))
     del keep
+
+  # -- slab gather (reindexing in time) ---------------------------------------
+  def slab_gather(self, src: int, src_dtype: int, src_elems: int, slab: int,
+                  nslab: int, offsets, out: int, out_dtype: int = F32):
+    """src and out are DEVICE addresses (wb2_slab_gather); offsets a host
+    int64 table of nslab source offsets, negative for a NaN slab."""
+    off = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+    check(self.lib.wb2_slab_gather(
+        self.handle, _P(src) if src else None, int(src_dtype), int(src_elems),
+        int(slab), int(nslab), _as_ptr(off, C.c_int64), _P(out) if out else None,
+        int(out_dtype)))
+
+  def slab_gather_host(self, src: int, src_dtype: int, src_elems: int,
+                       slab: int, nslab: int, offsets, budget: int, out: int,
+                       out_dtype: int = F32):
+    """src and out are HOST addresses (wb2_slab_gather_host)."""
+    off = np.ascontiguousarray(offsets, dtype=np.int64).reshape(-1)
+    check(self.lib.wb2_slab_gather_host(
+        self.handle, _P(src) if src else None, int(src_dtype), int(src_elems),
+        int(slab), int(nslab), _as_ptr(off, C.c_int64), int(budget),
+        _P(out) if out else None, int(out_dtype)))
 
   # -- K10 --------------------------------------------------------------------
   def rank_histogram(self, x: int, t: int, nmember: int, member_stride: int,
