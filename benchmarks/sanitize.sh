@@ -9,7 +9,7 @@
 OUT="${1:-$(mktemp -d)}"
 mkdir -p "$OUT"
 SEL='not fullsize and not full_size and not headline and not 721 and not m50 and not correlated and not k1_tma_scratch and not test_realistic_family and not long_time_sum and not claimed_instance'
-TESTS="tests/test_spectrum_pfa_gpu.py tests/test_spectrum_cases_gpu.py tests/test_regrid_tma_gpu.py tests/test_regrid_cases_gpu.py tests/test_det_metrics_gpu.py tests/test_host_streaming_gpu.py tests/test_ens_metrics_gpu.py tests/test_threshold_abi_gpu.py tests/test_wind_dynamics_gpu.py tests/test_region_reduce_gpu.py tests/test_precip_accumulation_gpu.py tests/test_column_integrals_gpu.py"
+TESTS="tests/test_spectrum_pfa_gpu.py tests/test_spectrum_cases_gpu.py tests/test_regrid_tma_gpu.py tests/test_regrid_cases_gpu.py tests/test_det_metrics_gpu.py tests/test_host_streaming_gpu.py tests/test_ens_metrics_gpu.py tests/test_threshold_abi_gpu.py tests/test_wind_dynamics_gpu.py tests/test_region_reduce_gpu.py tests/test_precip_accumulation_gpu.py tests/test_column_integrals_gpu.py tests/test_interp_cases_gpu.py"
 for tool in racecheck synccheck memcheck; do
   timeout 900 compute-sanitizer --tool $tool --print-limit 20 \
     python -m pytest $TESTS -x -q -m gpu -k "$SEL" -p no:cacheprovider \

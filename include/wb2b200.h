@@ -475,7 +475,10 @@ int wb2_ens_mean(wb2_ctx* ctx, const float* x, int32_t nmember,
  * of a spectrum lives on the increasing frequencies freq_table[lat][k] (host
  * [nrow][nk] float64, the `frequency` coordinate of the reference's result);
  * every row is interpolated linearly to the common `freqs` (host [nfreq],
- * float64), NaN outside the row's range like xarray's .interp.
+ * float64), NaN outside the row's range like xarray's .interp, with scipy
+ * interp1d's interval (searchsorted side='left') and weighted form
+ * ((f - x_lo) / dx) * y_hi + ((x_hi - f) / dx) * y_lo in float64: scipy's
+ * value rounded to float32, NaN / inf included.
  *   spec device [nfield][nrow][nk] float32;  out device [nfield][nrow][nfreq]    */
 int wb2_spectrum_interp(wb2_ctx* ctx, const float* spec, int64_t nfield,
                         int32_t nrow, int32_t nk, const double* freq_table,
@@ -853,9 +856,13 @@ int wb2_regrid_conservative_host(wb2_ctx* ctx, const float* src, float* dst,
  * into the raveled (lon, lat) source slab (BallTree / haversine nearest
  * neighbours, computed by the binder like regridding.py:212-228).
  * wb2_regrid_bilinear replaces BilinearRegridder.regrid_array (:256-294): per
- * target longitude a / latitude c two source taps and the fraction
- * delta / dx of jnp.interp (host arrays; tap -1 = NaN outside the source);
- * latitude is interpolated first, then longitude, in float32.
+ * target longitude a / latitude c two source taps i0, i1 and the fraction
+ * t = delta / dx of jnp.interp (host arrays): i0 = -1 is NaN (outside the
+ * source; i1 must then be -1 too); t < 0 returns fp[i0] untouched (jnp.interp's
+ * `where` at clamped ends and at |dx| <= spacing(eps); the binder passes
+ * i1 = i0, t = -1); otherwise fp[i0] + t * (fp[i1] - fp[i0]) with three
+ * separate float32 roundings.  Latitude is interpolated first, then longitude;
+ * taps outside [-1, n), or with only one of i0 / i1 at -1, are rejected.
  * Slabs are (lon, lat) with lat contiguous; strides in elements.               */
 int wb2_regrid_gather(wb2_ctx* ctx, const float* src, float* dst, int64_t nfield,
                       int64_t src_field_stride, int64_t dst_field_stride,

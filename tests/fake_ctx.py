@@ -489,8 +489,11 @@ class FakeContext:
       shape = [1, 1]
       shape[axis] = -1
       fr = np.asarray(frac, dtype=np.float32).reshape(shape)
-      val = lo + fr * (hi - lo)
-      outside = ((i0 < 0) | (i1 < 0)).reshape(shape)
+      with _quiet():
+        val = lo + fr * (hi - lo)
+      # t < 0: jnp.interp's `where` returns the tap value itself
+      val = np.where((fr < 0), lo, val)
+      outside = (i0 < 0).reshape(shape)
       return np.where(outside, np.float32(np.nan), val).astype(np.float32)
 
     for i in range(nfield):
@@ -566,10 +569,20 @@ class FakeContext:
     fr = np.asarray(freqs, dtype=np.float64)
     res = _view(out, nfield * nrow * fr.size, np.float32).reshape(
         nfield, nrow, fr.size)
-    for i in range(nfield):
-      for r in range(nrow):
-        res[i, r] = np.interp(fr, table[r], a[i, r].astype(np.float64),
-                              left=np.nan, right=np.nan)
+    # scipy interp1d's linear interval (searchsorted side='left', clipped) and
+    # weighted form in float64, like the kernel
+    for r in range(nrow):
+      x = table[r]
+      hi = np.clip(np.searchsorted(x, fr, side='left'), 1, nk - 1)
+      lo = hi - 1
+      dx = x[hi] - x[lo]
+      w_hi, w_lo = (fr - x[lo]) / dx, (x[hi] - fr) / dx
+      outside = ~((fr >= x[0]) & (fr <= x[-1]))
+      for i in range(nfield):
+        y = a[i, r].astype(np.float64)
+        with _quiet():
+          val = w_hi * y[hi] + w_lo * y[lo]
+        res[i, r] = np.where(outside, np.nan, val)
 
   def __getattr__(self, name):
     raise AttributeError(

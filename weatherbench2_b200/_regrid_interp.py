@@ -17,6 +17,7 @@ from weatherbench2_b200 import _lib
 from weatherbench2_b200 import regridding as rg
 
 _F32 = np.float32  # JAX default precision (x64 off) of the reference
+_TAP = _F32(-1)    # fraction of a tap jnp.interp returns as it is
 
 
 def nearest_neighbor_indices(source_grid: 'rg.Grid', target_grid: 'rg.Grid'
@@ -37,21 +38,35 @@ def nearest_neighbor_indices(source_grid: 'rg.Grid', target_grid: 'rg.Grid'
   return tree.query(points(target_grid), k=1, return_distance=False)[:, 0]
 
 
+def _jnp_remainder(x, period):
+  """`x % period` as jnp.remainder computes it: C fmod, plus `period` where the
+  nonzero remainder has the other sign (-0.0 stays -0.0, unlike np.mod)."""
+  r = np.fmod(x, period)
+  return np.where((r != 0) & ((r < 0) != (period < 0)), r + period,
+                  r).astype(x.dtype)
+
+
 def interp_taps(x, xp, clamp: bool, period: Optional[float] = None):
   """Taps of `jnp.interp(x, xp, fp, left, right, period)` in float32:
-  (i0, i1, t) such that f = fp[i0] + t * (fp[i1] - fp[i0]); i0 = -1 where the
-  result is NaN (outside `xp` when `clamp` is False).  `clamp` is jnp.interp's
-  default (left = fp[0], right = fp[-1])."""
+  (i0, i1, t) such that f = fp[i0] + t * (fp[i1] - fp[i0]).  i0 = -1 where the
+  result is NaN (outside `xp` when `clamp` is False), with i1 = -1 too.  Where
+  jnp.interp returns a tap value through `where` -- fp[0] / fp[-1] outside `xp`
+  when `clamp` is True (jnp.interp's default left / right), fp[i-1] where
+  |dx| <= spacing(eps) -- the taps are i1 = i0 and t = -1, and the kernel passes
+  fp[i0] through untouched.  A genuine fraction is never negative, and
+  `i0 == i1` alone does not mean a `where`: a one-longitude periodic axis has
+  i0 == i1 == 0 and t = x / 360, and jnp.interp lerps there too.  Read as a
+  plain lerp, fp + (-1) * (fp - fp) is still fp for every finite tap."""
   x = np.asarray(x, dtype=_F32)
   xp = np.asarray(xp, dtype=_F32)
   n = xp.size
   if period is not None:
-    x = np.mod(x, _F32(period))
-    xp_m = np.mod(xp, _F32(period))
+    p = np.abs(_F32(period))
+    x = _jnp_remainder(x, p)
+    xp_m = _jnp_remainder(xp, p)
     order = np.argsort(xp_m, kind='stable')
     xp_s = xp_m[order]
-    xp_ext = np.concatenate([xp_s[-1:] - _F32(period), xp_s,
-                             xp_s[:1] + _F32(period)]).astype(_F32)
+    xp_ext = np.concatenate([xp_s[-1:] - p, xp_s, xp_s[:1] + p]).astype(_F32)
     src = np.concatenate([order[-1:], order, order[:1]])
   else:
     xp_ext, src = xp, np.arange(n)
@@ -60,15 +75,15 @@ def interp_taps(x, xp, clamp: bool, period: Optional[float] = None):
   delta = (x - xp_ext[i - 1]).astype(_F32)
   eps = np.spacing(np.finfo(_F32).eps)
   dx0 = np.abs(dx) <= eps
-  t = np.where(dx0, _F32(0), delta / np.where(dx0, _F32(1), dx)).astype(_F32)
+  t = np.where(dx0, _TAP, delta / np.where(dx0, _F32(1), dx)).astype(_F32)
   i0 = src[i - 1].astype(np.int32)
-  i1 = np.where(dx0, src[i - 1], src[i]).astype(np.int32)
+  i1 = np.where(dx0, i0, src[i]).astype(np.int32)
   if period is None:
     lo, hi = x < xp[0], x > xp[-1]
     if clamp:
       i0 = np.where(lo, 0, np.where(hi, n - 1, i0)).astype(np.int32)
-      i1 = np.where(lo, 0, np.where(hi, n - 1, i1)).astype(np.int32)
-      t = np.where(lo | hi, _F32(0), t).astype(_F32)
+      i1 = np.where(lo | hi, i0, i1).astype(np.int32)
+      t = np.where(lo | hi, _TAP, t).astype(_F32)
     else:
       i0 = np.where(lo | hi, -1, i0).astype(np.int32)
       i1 = np.where(lo | hi, -1, i1).astype(np.int32)

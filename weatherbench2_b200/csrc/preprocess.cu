@@ -11,9 +11,15 @@
 // (weatherbench2/derived_variables.py:629-682): every latitude row of a zonal
 // spectrum lives on its own frequency axis f_k = k / (L * spacing(lat)) (passed
 // as a table, the reference's own coordinate values); the rows are
-// interpolated linearly to common frequencies, NaN outside the row's range (xarray .interp -> scipy interp1d(bounds_error=False)).  The slope
-// form y0 + (y1 - y0) / (x1 - x0) * (x - x0) and float64 arithmetic follow
-// scipy's linear interp1d.
+// interpolated linearly to common frequencies, NaN outside the row's range
+// (xarray .interp -> scipy interp1d(bounds_error=False)).  The interval and the
+// formula are scipy's linear interp1d (_call_linear): lo = clip(searchsorted(x,
+// f, side='left'), 1, nk - 1) - 1, so a node x[k] > x[0] is reached from the
+// interval below it, and
+//     y = ((f - x_lo) / dx) * y_hi + ((x_hi - f) / dx) * y_lo,   dx = x_hi - x_lo
+// in float64 with every operation rounded on its own (no FMA contraction).  The
+// float64 value is therefore scipy's bit for bit and the float32 result its
+// rounding; NaN / inf propagate exactly as in scipy (0 * inf = NaN included).
 #include <algorithm>
 
 #include "common.cuh"
@@ -93,15 +99,18 @@ __global__ void __launch_bounds__(256) spectrum_interp_kernel(
     if (f >= x[0] && f <= x[nk - 1]) {
       // the axis is uniform in k: guess the interval, then settle on the table
       // values themselves (the coordinates are the reference's, not k * step)
+      // to the largest lo with x[lo] < f (0 when f == x[0])
       const double step = x[1] - x[0];
-      int k0 = step > 0.0 ? static_cast<int>(floor((f - x[0]) / step)) : 0;
-      k0 = max(0, min(k0, nk - 2));
-      while (k0 < nk - 2 && x[k0 + 1] < f) ++k0;
-      while (k0 > 0 && x[k0] > f) --k0;
-      const double x0 = x[k0], x1 = x[k0 + 1];
-      const double y0 = double(spec[fr * nk + k0]), y1 = double(spec[fr * nk + k0 + 1]);
-      const double slope = (y1 - y0) / (x1 - x0);
-      r = static_cast<float>(slope * (f - x0) + y0);
+      int lo = step > 0.0 ? static_cast<int>(floor((f - x[0]) / step)) : 0;
+      lo = max(0, min(lo, nk - 2));
+      while (lo < nk - 2 && x[lo + 1] < f) ++lo;
+      while (lo > 0 && x[lo] >= f) --lo;
+      const double x_lo = x[lo], x_hi = x[lo + 1];
+      const double y_lo = double(spec[fr * nk + lo]), y_hi = double(spec[fr * nk + lo + 1]);
+      const double dx = __dsub_rn(x_hi, x_lo);
+      const double w_hi = __ddiv_rn(__dsub_rn(f, x_lo), dx);
+      const double w_lo = __ddiv_rn(__dsub_rn(x_hi, f), dx);
+      r = __double2float_rn(__dadd_rn(__dmul_rn(w_hi, y_hi), __dmul_rn(w_lo, y_lo)));
     }
     out[i] = r;
   }

@@ -9,8 +9,18 @@
 // 1-D linear interpolations with jnp.interp's formula
 //     f = fp[i-1] + (delta / dx) * (fp[i] - fp[i-1])
 // first along latitude, then along longitude, in float32 like JAX.  The host
-// resolves searchsorted / clamping / periodic wrap-around / "NaN outside" into
-// two taps and a fraction per target coordinate.
+// resolves x % period / the stable key sort / searchsorted / the clip into two
+// taps and the fraction t = delta / dx per target coordinate (i0 = -1: NaN, the
+// left = right = nan `where`s).  jnp.interp's other `where`s -- fp[0] / fp[-1]
+// outside a clamped axis, fp[i-1] where |dx| <= spacing(eps) -- return the tap
+// value itself; the host marks them i1 = i0, t = -1 and the kernel passes
+// fp[i0] through untouched, so an infinite tap stays infinite (fp + 0 * (fp - fp)
+// would be NaN).  A genuine fraction is never negative (it lies in [0, 1], -0.0
+// at most), and i1 = i0 with t = -1 read as a plain lerp still gives
+// fp + (-1) * 0 = fp bit for bit for every finite tap, -0.0 included.
+// Each lerp is three separately rounded operations (no FMA contraction), so
+// given the host's taps the result is bit-equal to a float32 transcription of
+// jnp.interp applied in the reference's order.
 //
 // Fields are (lon, lat) slabs like the conservative regridder's.  Both kernels
 // are gathers: 4 B written per target cell, 4 (nearest) or 16 (bilinear) bytes
@@ -22,6 +32,11 @@
 namespace wb2 {
 
 constexpr int kInterpThreads = 256;
+
+// jnp.interp's a + t * (b - a), each operation rounded on its own
+__device__ __forceinline__ float lerp_rn(float a, float b, float t) {
+  return __fadd_rn(a, __fmul_rn(t, __fsub_rn(b, a)));
+}
 
 __global__ void __launch_bounds__(kInterpThreads)
     regrid_gather_kernel(const float* __restrict__ src, float* __restrict__ dst,
@@ -37,8 +52,8 @@ struct BilinearParams {
   const float* src;
   float* dst;
   const int32_t* lon_i0;  // [nlon_t] source longitude index of the left tap, -1: NaN
-  const int32_t* lon_i1;
-  const float* lon_t;     // [nlon_t] delta / dx
+  const int32_t* lon_i1;  // right tap (-1 exactly where lon_i0 is)
+  const float* lon_t;     // [nlon_t] delta / dx; < 0: fp[lon_i0] exactly
   const int32_t* lat_i0;  // [nlat_t]
   const int32_t* lat_i1;
   const float* lat_t;
@@ -58,15 +73,15 @@ __global__ void __launch_bounds__(kInterpThreads) regrid_bilinear_kernel(const B
   if (b0 >= 0 && d0 >= 0) {
     const float* s = p.src + field * p.src_stride;
     const float tl = p.lat_t[c], tn = p.lon_t[a];
-    // latitude first (regridding.py:262-274), on the two longitude taps
+    // latitude first (regridding.py:262-274), on the two longitude taps; a
+    // negative fraction returns the i0 tap itself (jnp.interp's `where`)
     const float x00 = __ldg(s + int64_t(b0) * p.nlat_s + d0);
     const float x01 = __ldg(s + int64_t(b0) * p.nlat_s + d1);
     const float x10 = __ldg(s + int64_t(b1) * p.nlat_s + d0);
     const float x11 = __ldg(s + int64_t(b1) * p.nlat_s + d1);
-    const float y0 = __fadd_rn(x00, __fmul_rn(tl, __fsub_rn(x01, x00)));
-    const float y1 = __fadd_rn(x10, __fmul_rn(tl, __fsub_rn(x11, x10)));
-    // then longitude (:276-292)
-    out = __fadd_rn(y0, __fmul_rn(tn, __fsub_rn(y1, y0)));
+    const float y0 = tl < 0.f ? x00 : lerp_rn(x00, x01, tl);
+    const float y1 = tl < 0.f ? x10 : lerp_rn(x10, x11, tl);
+    out = tn < 0.f ? y0 : lerp_rn(y0, y1, tn);  // then longitude (:276-292)
   }
   p.dst[field * p.dst_stride + k] = out;
 }
@@ -118,10 +133,12 @@ extern "C" int wb2_regrid_bilinear(wb2_ctx* ctx, const float* src, float* dst, i
   WB2_REQUIRE(src && dst && lon_i0 && lon_i1 && lon_t && lat_i0 && lat_i1 && lat_t,
               "NULL argument");
   for (int32_t a = 0; a < nlon_t; ++a)
-    WB2_REQUIRE(lon_i0[a] >= -1 && lon_i0[a] < nlon_s && lon_i1[a] >= -1 && lon_i1[a] < nlon_s,
+    WB2_REQUIRE(lon_i0[a] >= -1 && lon_i0[a] < nlon_s && lon_i1[a] >= -1 && lon_i1[a] < nlon_s &&
+                    (lon_i0[a] < 0) == (lon_i1[a] < 0),
                 "longitude tap %d out of range", a);
   for (int32_t c = 0; c < nlat_t; ++c)
-    WB2_REQUIRE(lat_i0[c] >= -1 && lat_i0[c] < nlat_s && lat_i1[c] >= -1 && lat_i1[c] < nlat_s,
+    WB2_REQUIRE(lat_i0[c] >= -1 && lat_i0[c] < nlat_s && lat_i1[c] >= -1 && lat_i1[c] < nlat_s &&
+                    (lat_i0[c] < 0) == (lat_i1[c] < 0),
                 "latitude tap %d out of range", c);
   DeviceGuard guard(ctx->device);
   Packer pk(ctx);
