@@ -267,18 +267,25 @@ int wb2_ens_maps(wb2_ctx* ctx, const void* x, const void* t, int dtype,
  * and truth precipitation, the 3 x 3 scoring matrix of the cell's
  * climatological dry fraction p1, NaN where p1 is outside (min_p1, max_p1).
  * SEEPS (the spatial mean with skipna, :516-528) is wb2_det_metrics on the maps.
- *   wet          device base of the climatological wet-threshold slabs;
+ * Every operand is read in its own dtype and each comparison runs in NumPy's
+ * promoted dtype: dry_threshold is rounded to f's / t's dtype, min_p1 / max_p1
+ * to p1's, and the scoring matrix is formed in p1's dtype.  The maps are
+ * float32(reference).
+ *   f, t         device precipitation of f_dtype / t_dtype (WB2_F32 / WB2_F64)
+ *   wet          device base of the climatological wet-threshold slabs, of
+ *                wet_dtype;
  *   off_wet_f/t  host [nout * ngroup]: the slab for the forecast's / truth's
  *                valid time (day-of-year / hour lookup folded into the table)
- *   p1           device [nrow][ncol] float32 mean dry fraction
+ *   p1           device [nrow][ncol] mean dry fraction of p1_dtype
  *   out          device [nout][nrow][ncol] float32                               */
-int wb2_seeps_maps(wb2_ctx* ctx, const float* f, const float* t, const float* wet,
-                   const float* p1, int64_t nout, int32_t ngroup,
+int wb2_seeps_maps(wb2_ctx* ctx, const void* f, int f_dtype, const void* t, int t_dtype,
+                   const void* wet, int wet_dtype, const void* p1, int p1_dtype,
+                   int64_t nout, int32_t ngroup,
                    const int64_t* off_f, const int64_t* off_t,
                    const int64_t* off_wet_f, const int64_t* off_wet_t,
                    int32_t nrow, int32_t ncol, int64_t row_stride,
-                   int64_t wet_row_stride, float dry_threshold, float min_p1,
-                   float max_p1, int skipna, float* out);
+                   int64_t wet_row_stride, double dry_threshold, double min_p1,
+                   double max_p1, int skipna, float* out);
 
 /* ---- derived variables -------------------------------------------------------------
  * wb2_wind_speed replaces WindSpeed.compute (derived_variables.py:77-99):

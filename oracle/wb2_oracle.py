@@ -937,11 +937,17 @@ def bilinear_regrid(field, source: Grid, target: Grid):
 # SEEPS -- metrics.py:417-528.
 # ---------------------------------------------------------------------------
 def seeps_pointwise(f, t, wet_f, wet_t, p1, dry_threshold_mm=0.25, min_p1=0.1,
-                    max_p1=0.85):
+                    max_p1=0.85, dry_threshold=None):
   """SpatialSEEPS.compute_chunk on arrays that broadcast against each other:
   f / t precipitation, wet_f / wet_t the climatological wet threshold at their
-  valid times, p1 the mean dry fraction."""
-  dry_threshold = dry_threshold_mm / 1000.0
+  valid times, p1 the mean dry fraction.  Every operation runs in NumPy's
+  promoted dtype, as in the reference: the Python-float thresholds are weak
+  scalars, rounded to the dtype of the array they meet.  `dry_threshold` (in
+  metres) replaces dry_threshold_mm / 1000 when given."""
+  if dry_threshold is None:
+    dry_threshold = dry_threshold_mm / 1000.0
+  dry_threshold, min_p1, max_p1 = (float(dry_threshold), float(min_p1),
+                                    float(max_p1))
 
   def cats(x, wet):  # metrics.py:446-460
     dry = x < dry_threshold

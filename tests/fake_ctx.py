@@ -384,13 +384,17 @@ class FakeContext:
   # -- K9: SEEPS maps --------------------------------------------------------------
   def seeps_maps(self, f, t, wet, p1, nout, ngroup, off_f, off_t, off_wet_f,
                  off_wet_t, nrow, ncol, row_stride, wet_row_stride,
-                 dry_threshold, min_p1, max_p1, skipna, out):
+                 dry_threshold, min_p1, max_p1, skipna, out, *,
+                 f_dtype=_lib.F32, t_dtype=_lib.F32, wet_dtype=_lib.F32,
+                 p1_dtype=_lib.F32):
+    """The reference on the operands in their own dtypes, averaged in float64
+    and rounded once to float32, as the kernel documents."""
     from oracle import wb2_oracle as orc  # pylint: disable=import-outside-toplevel
     self.calls.append(('seeps_maps', int(nout), int(ngroup)))
+    dt = {_lib.F32: np.float32, _lib.F64: np.float64}
     g = self._geometry(nrow, ncol, row_stride)
     gw = self._geometry(nrow, ncol, wet_row_stride)
-    p1a = _view(p1, nrow * ncol, np.float32).reshape(nrow, ncol).astype(
-        np.float64)
+    p1a = _view(p1, nrow * ncol, dt[p1_dtype]).reshape(nrow, ncol).copy()
     res = np.empty((nout, nrow, ncol), dtype=np.float32)
     for j in range(nout):
       terms = []
@@ -398,11 +402,12 @@ class FakeContext:
         i = j * ngroup + q
         with _quiet():
           terms.append(orc.seeps_pointwise(
-              _slab(f, off_f[i], g, np.float32),
-              _slab(t, off_t[i], g, np.float32),
-              _slab(wet, off_wet_f[i], gw, np.float32),
-              _slab(wet, off_wet_t[i], gw, np.float32), p1a,
-              float(dry_threshold) * 1000.0, float(min_p1), float(max_p1)))
+              _slab(f, off_f[i], g, dt[f_dtype], native=True),
+              _slab(t, off_t[i], g, dt[t_dtype], native=True),
+              _slab(wet, off_wet_f[i], gw, dt[wet_dtype], native=True),
+              _slab(wet, off_wet_t[i], gw, dt[wet_dtype], native=True), p1a,
+              min_p1=float(min_p1), max_p1=float(max_p1),
+              dry_threshold=float(dry_threshold)))
       with _quiet():
         res[j] = (np.nanmean if skipna else np.mean)(np.stack(terms), axis=0)
     _view(out, res.size, np.float32)[...] = res.reshape(-1)

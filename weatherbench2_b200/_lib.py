@@ -146,9 +146,10 @@ PROTOTYPES = {
         C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_uint64,
         _P]),
     'wb2_seeps_maps': (C.c_int, [
-        _P, _P, _P, _P, _P, C.c_int64, C.c_int32, _I64P, _I64P, _I64P, _I64P,
-        C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_float, C.c_float,
-        C.c_float, C.c_int, _P]),
+        _P, _P, C.c_int, _P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_int64,
+        C.c_int32, _I64P, _I64P, _I64P, _I64P, C.c_int32, C.c_int32,
+        C.c_int64, C.c_int64, C.c_double, C.c_double, C.c_double, C.c_int,
+        _P]),
     'wb2_regrid_gather': (C.c_int, [_P, _P, _P, C.c_int64, C.c_int64, C.c_int64,
                                     C.c_int32, C.c_int32,
                                     C.POINTER(C.c_int32)]),
@@ -944,12 +945,18 @@ class Context:
                  off_wet_f: np.ndarray, off_wet_t: np.ndarray, nrow: int,
                  ncol: int, row_stride: int, wet_row_stride: int,
                  dry_threshold: float, min_p1: float, max_p1: float,
-                 skipna: bool, out: int):
+                 skipna: bool, out: int, *, f_dtype: int = F32,
+                 t_dtype: int = F32, wet_dtype: int = F32,
+                 p1_dtype: int = F32):
+    """K9.  The *_dtype keywords are F32 (the default) or F64, one per
+    operand; the three thresholds are Python floats, rounded by the kernel to
+    the dtype they are compared in."""
     n = nout * ngroup
     assert off_f.size == n and off_t.size == n
     assert off_wet_f.size == n and off_wet_t.size == n
     check(self.lib.wb2_seeps_maps(
-        self.handle, _P(f), _P(t), _P(wet), _P(p1), int(nout), int(ngroup),
+        self.handle, _P(f), int(f_dtype), _P(t), int(t_dtype), _P(wet),
+        int(wet_dtype), _P(p1), int(p1_dtype), int(nout), int(ngroup),
         _as_ptr(off_f, C.c_int64), _as_ptr(off_t, C.c_int64),
         _as_ptr(off_wet_f, C.c_int64), _as_ptr(off_wet_t, C.c_int64),
         int(nrow), int(ncol), int(row_stride), int(wet_row_stride),

@@ -74,9 +74,15 @@ class SpatialSEEPS(m.Metric):
     name = self.precip_name
     f_da, t_da = xl.align_inner(forecast[name], truth[name])
     wet_da = clim[f'{name}_seeps_threshold']
-    f_op = sp.prepare_operand(f_da, None, np.float32)
-    t_op = sp.prepare_operand(t_da, f_op.layout, np.float32)
-    w_op = sp.prepare_operand(wet_da, f_op.layout, np.float32)
+    for da in (f_da, t_da, wet_da):
+      if da.dtype not in (np.float32, np.float64):
+        raise TypeError(f'variable {da.name!r} has dtype {da.dtype}: SEEPS '
+                        'takes float32 or float64 data')
+    # each operand keeps its dtype: the kernel categorises in NumPy's
+    # promoted precision, as the reference does (metrics.py:456-460)
+    f_op = sp.prepare_operand(f_da, None)
+    t_op = sp.prepare_operand(t_da, f_op.layout)
+    w_op = sp.prepare_operand(wet_da, f_op.layout)
     maps, dims = sp.run_seeps_maps(
         ctx, f_op, t_op, w_op, _threshold_maps(wet_da, f_da),
         _threshold_maps(wet_da, t_da), self.p1, self.dry_threshold_mm / 1000.0,

@@ -845,12 +845,31 @@ def run_seeps_maps(ctx: _lib.Context, f_op: Operand, t_op: Operand,
   `reduce_dim`.  The wet thresholds `wet_op` are looked up at the forecast's
   and the truth's valid times through the `gather_operand` index maps
   `f_lookup` / `t_lookup`; `p1` is the (latitude, longitude) DataArray of the
-  average dry fraction.  Returns (maps, dims)."""
-  p1 = np.ascontiguousarray(np.asarray(p1.transpose(*_map_dims(f_op)).values),
-                            dtype=np.float32)
+  average dry fraction.  Every operand keeps its dtype (float32 or float64):
+  the kernel compares in NumPy's promoted dtype, as the reference does.
+  Returns (maps, dims)."""
+  p1 = np.asarray(p1.transpose(*_map_dims(f_op)).values)
+  for what, dt in (('forecast', f_op.dtype), ('truth', t_op.dtype),
+                   ('wet threshold', wet_op.dtype), ('dry fraction', p1.dtype)):
+    if dt not in (np.float32, np.float64):
+      raise TypeError(f'SEEPS takes float32 or float64 data; the {what} is '
+                      f'{dt}')
+  p1 = np.ascontiguousarray(p1)
   if p1.shape != (f_op.nrow, f_op.ncol):
     raise ValueError(f'dry fraction grid {p1.shape} does not match the '
                      f'data grid {(f_op.nrow, f_op.ncol)}')
+  # The Python-float thresholds are weak scalars: rounded to the dtype they
+  # are compared in, the dry threshold to the precipitation's (the kernel
+  # rounds it again for a float32 side of a mixed pair, which changes
+  # nothing) and the p1 bounds to p1's.  Only float64 operands are named, so
+  # an all-float32 launch makes the same Context call, with the same values,
+  # as before the dtype codes existed.
+  dry_threshold = float(np.result_type(f_op.dtype, t_op.dtype).type(
+      dry_threshold))
+  min_p1, max_p1 = (float(p1.dtype.type(v)) for v in (min_p1, max_p1))
+  dtypes = {f'{k}_dtype': _lib.F64 for k, dt in (
+      ('f', f_op.dtype), ('t', t_op.dtype), ('wet', wet_op.dtype),
+      ('p1', p1.dtype)) if dt == np.float64}
   with Staging(ctx) as stage:
     f_op, t_op, wet_op = (stage.upload(op) for op in (f_op, t_op, wet_op))
     _check_grid([f_op, t_op])
@@ -867,8 +886,8 @@ def run_seeps_maps(ctx: _lib.Context, f_op: Operand, t_op: Operand,
         lambda out: ctx.seeps_maps(
             f_op.addr, t_op.addr, wet_op.addr, p1_dev, tabs[0].size // ngroup,
             ngroup, *tabs, f_op.nrow, f_op.ncol, f_op.row_stride,
-            wet_op.row_stride, np.float32(dry_threshold), np.float32(min_p1),
-            np.float32(max_p1), skipna, out))
+            wet_op.row_stride, float(dry_threshold), float(min_p1),
+            float(max_p1), skipna, out, **dtypes))
   return maps, out_dims + _map_dims(f_op)
 
 
