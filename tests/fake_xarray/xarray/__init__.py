@@ -70,32 +70,3 @@ class Dataset:
   def __getitem__(self, k):
     return self.data_vars[k]
 
-  def keys(self):
-    return self.data_vars.keys()
-
-  @property
-  def dims(self):
-    out = {}
-    for v in self.data_vars.values():
-      out.update(dict(zip(v.dims, v.shape)))
-    return out
-
-  sizes = dims
-
-  def mean(self, dim, skipna=None):
-    fn = np.nanmean if skipna else np.mean
-    out = {}
-    for k, v in self.data_vars.items():
-      if dim not in v.dims:
-        out[k] = v
-        continue
-      ax = v.dims.index(dim)
-      dims = v.dims[:ax] + v.dims[ax + 1:]
-      out[k] = DataArray(fn(v.data, axis=ax), dims,
-                         {c: cc for c, cc in v.coords.items()
-                          if dim not in cc.dims}, k, v.attrs)
-    coords = {c: cc for c, cc in self.coords.items() if dim not in cc.dims}
-    return Dataset(out, coords, self.attrs)
-
-  def assign_attrs(self, **kw):
-    return Dataset(self.data_vars, self.coords, dict(self.attrs, **kw))

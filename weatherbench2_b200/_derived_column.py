@@ -4,10 +4,10 @@ integrated water transport and eddy kinetic energy, computed on the device
 (csrc/column_integral.cu).  Imported into `weatherbench2_b200.derived_variables`.
 
 A CUDA operand gives a CUDA tensor on its device, which the metric kernels
-read in place; NumPy, memmap or lazily gathered input gives NumPy; native
-xarray gives native xarray.  Float32 data gives float32, float64 gives
-float64.  The result has the input's dims without `level`, in the same order,
-and the input's coords without those along `level`, as xarray's integrate.
+read in place; NumPy, memmap or lazily gathered input gives NumPy.  Float32
+data gives float32, float64 gives float64.  The result has the input's dims
+without `level`, in the same order, and the input's coords without those along
+`level`, as xarray's integrate.
 Numerics and deviations: include/wb2b200.h and DESIGN.md section 8h.
 """
 from __future__ import annotations
@@ -39,9 +39,7 @@ def column_integral(dataset, kind: int, names: t.Sequence[str],
   TOTAL_COLUMN; q, u, v for IVT; u, v for EKE).  `level_slice` selects the
   levels as `.sel(level=level_slice)`: a contiguous run, passed to the kernel
   as a pointer offset and a count."""
-  native = xl.is_native_xarray(dataset)
-  ds = xl.from_xarray(dataset)
-  das = [ds[n] for n in names]  # KeyError for a missing base variable
+  das = [dataset[n] for n in names]  # KeyError for a missing base variable
   ref = das[0]
   for name, da in zip(names, das):
     if 'level' not in da.dims:
@@ -107,8 +105,6 @@ def column_integral(dataset, kind: int, names: t.Sequence[str],
     result = result.transpose(*ref_dims)
     if xl._is_torch(result.data):  # pylint: disable=protected-access
       result = xl.DataArray(result.data.contiguous(), ref_dims, coords)
-  if native:
-    return xl.to_xarray(xl.Dataset({'_': result}))['_']
   return result
 
 

@@ -23,13 +23,6 @@ from weatherbench2_b200 import resampling
 from weatherbench2_b200 import xarray_lite as xl
 
 
-def _wrap(src, da: xl.DataArray, values):
-  result = xl.DataArray(values, da.dims, dict(da.coords), da.name, da.attrs)
-  if xl.is_native_xarray(src):
-    return xl.to_xarray(xl.Dataset({'_': result}))['_']
-  return result
-
-
 def _lead_values(ds, da: xl.DataArray, lead: str) -> np.ndarray:
   if lead in da.coords:
     return np.asarray(da.coords[lead].values)
@@ -105,15 +98,14 @@ class PrecipitationAccumulation(dv.DerivedVariable):
     return int(steps)
 
   def compute(self, dataset):
-    ds = xl.from_xarray(dataset)
-    da = ds[self.total_precipitation_name]
+    da = dataset[self.total_precipitation_name]
     if self.lead_time_name not in da.dims:
       raise ValueError(f'{self.total_precipitation_name!r} has no '
                        f'{self.lead_time_name!r} dimension')
-    w = self.window(_lead_values(ds, da, self.lead_time_name))
+    w = self.window(_lead_values(dataset, da, self.lead_time_name))
     values = precip_accumulation(da, self.lead_time_name, w,
                                  self.set_negative_to_zero)
-    return _wrap(dataset, da, values)
+    return xl.DataArray(values, da.dims, da.coords, da.name, da.attrs)
 
 
 @dataclasses.dataclass
@@ -138,8 +130,7 @@ class AggregatePrecipitationAccumulation(dv.DerivedVariable):
     return ([self.lead_time_name],), [self.lead_time_name]
 
   def compute(self, dataset):
-    ds = xl.from_xarray(dataset)
-    da = ds[self.raw_accumulation_name]
+    da = dataset[self.raw_accumulation_name]
     steps = float(np.timedelta64(self.accumulation_hours, 'h') /
                   np.timedelta64(self.raw_accumulation_hours, 'h'))
     if not steps.is_integer():
@@ -152,4 +143,4 @@ class AggregatePrecipitationAccumulation(dv.DerivedVariable):
                        f'{self.lead_time_name!r} dimension')
     values = resampling._stats(da, self.lead_time_name, ['sum'], skipna=False,  # pylint: disable=protected-access
                                window=int(steps))['sum']
-    return _wrap(dataset, da, values)
+    return xl.DataArray(values, da.dims, da.coords, da.name, da.attrs)

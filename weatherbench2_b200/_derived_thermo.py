@@ -5,10 +5,10 @@ relative humidity, computed on the device (csrc/thermo.cu).  Imported into
 
 A CUDA operand gives a CUDA tensor on its device, which the metric kernels
 read in place; NumPy, memmap or lazily gathered input is read once as NumPy
-and gives NumPy; native xarray gives native xarray.  An operand in another dim
-order is permuted to the order of the one whose dims the result takes:
-temperature's for the lapse rate, specific humidity's for the relative
-humidity, as xarray's `dT_dp / dz_dp` and `mixing_ratio / smr` order them.
+and gives NumPy.  An operand in another dim order is permuted to the order of
+the one whose dims the result takes: temperature's for the lapse rate,
+specific humidity's for the relative humidity, as xarray's `dT_dp / dz_dp`
+and `mixing_ratio / smr` order them.
 Operands whose dims or sizes differ raise ValueError, where xarray would align
 them.  Numerics and deviations: include/wb2b200.h and DESIGN.md section 8i.
 """
@@ -61,25 +61,16 @@ def _split(shape, axis):
   return nouter, shape[axis], ninner
 
 
-def _result(data, dims, coords, native):
-  result = xl.DataArray(data, dims, coords)
-  if native:
-    return xl.to_xarray(xl.Dataset({'_': result}))['_']
-  return result
-
-
 def lapse_rate(dataset, temperature_name: str, geopotential_name: str):
   """One wb2_lapse_rate call: dT/dlevel / ((1 / 9.81) dZ/dlevel) with
   np.gradient's arithmetic along `level`, in temperature's dims."""
-  native = xl.is_native_xarray(dataset)
-  ds = xl.from_xarray(dataset)
   names = [temperature_name, geopotential_name]
-  das, datas, perms, dtype = _operands(ds, names)
+  das, datas, perms, dtype = _operands(dataset, names)
   temp = das[0]
   if 'level' not in temp.dims:
     raise ValueError(f'{temperature_name!r} has no "level" dimension')
   level = (temp.coords['level'] if 'level' in temp.coords
-           else ds.coords.get('level'))
+           else dataset.coords.get('level'))
   if level is None or tuple(level.dims) != ('level',):
     raise ValueError('Coordinate level does not exist.')
   coef, uniform = _derived_wind.gradient_table(level.values)  # ValueError: < 2
@@ -97,7 +88,7 @@ def lapse_rate(dataset, temperature_name: str, geopotential_name: str):
                               perms=perms, dtype=dtype)
   coords = dict(das[1].coords)
   coords.update(temp.coords)
-  return _result(data, dims, coords, native)
+  return xl.DataArray(data, dims, coords)
 
 
 def relative_humidity(dataset, temperature_name: str,
@@ -105,14 +96,12 @@ def relative_humidity(dataset, temperature_name: str,
   """One wb2_relative_humidity call: MetPy's relative humidity from specific
   humidity with Bolton's saturation vapour pressure, T in K and the pressure
   coordinate in hPa, in specific humidity's dims."""
-  native = xl.is_native_xarray(dataset)
-  ds = xl.from_xarray(dataset)
   names = [specific_humidity_name, temperature_name]  # q first: its dims
-  das, datas, perms, dtype = _operands(ds, names)
+  das, datas, perms, dtype = _operands(dataset, names)
   q = das[0]
-  if pressure_name not in ds.coords:
+  if pressure_name not in dataset.coords:
     raise KeyError(pressure_name)
-  pcoord = ds.coords[pressure_name]
+  pcoord = dataset.coords[pressure_name]
   pvalues = np.asarray(pcoord.values)
   if len(pcoord.dims) > 1:
     raise ValueError(f'pressure coordinate {pressure_name!r} has dims '
@@ -150,7 +139,7 @@ def relative_humidity(dataset, temperature_name: str,
   coords.update(q.coords)
   if pressure_name not in coords:
     coords[pressure_name] = pcoord
-  return _result(data, dims, coords, native)
+  return xl.DataArray(data, dims, coords)
 
 
 @dataclasses.dataclass

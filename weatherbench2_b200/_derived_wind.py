@@ -40,9 +40,7 @@ class WindSpeed(_WindVariable):
     return ([], []), []
 
   def compute(self, dataset):
-    native = xl.is_native_xarray(dataset)
-    ds = xl.from_xarray(dataset)
-    u, v = ds[self.u_name], ds[self.v_name]
+    u, v = dataset[self.u_name], dataset[self.v_name]
     if u.dims != v.dims or u.shape != v.shape:
       v = v.transpose(*u.dims)
       if u.shape != v.shape:
@@ -53,10 +51,7 @@ class WindSpeed(_WindVariable):
         [u.data, v.data], [(u.shape, np.float32)],
         lambda i, o: ctx.wind_speed(i[0], i[1], o[0], n), dtype=np.float32)
     coords = {k: c for k, c in u.coords.items()}
-    result = xl.DataArray(data, u.dims, coords)
-    if native:
-      return xl.to_xarray(xl.Dataset({'_': result}))['_']
-    return result
+    return xl.DataArray(data, u.dims, coords)
 
 
 # ---- horizontal derivatives (derived_variables.py:102-338) -------------------
@@ -111,10 +106,8 @@ def wind_dynamics(dataset, kind: int, u_name=None, v_name=None, z_name=None):
   result keeps the first input's dims and coords; float32, on the device when
   an input is a CUDA tensor, else NumPy.  Float64 data is cast to float32 and
   float32 coordinates are taken as float64 (DESIGN.md, "Wind dynamics")."""
-  native = xl.is_native_xarray(dataset)
-  ds = xl.from_xarray(dataset)
   names = [n for n in (u_name, v_name, z_name) if n is not None]
-  das = [ds[n] for n in names]  # KeyError for a missing base variable
+  das = [dataset[n] for n in names]  # KeyError for a missing base variable
   ref = das[0]
   for d in ('latitude', 'longitude'):
     if d not in ref.dims or d not in ref.coords:
@@ -161,8 +154,6 @@ def wind_dynamics(dataset, kind: int, u_name=None, v_name=None, z_name=None):
   result = xl.DataArray(data, work, coords).transpose(*ref.dims)
   if xl._is_torch(result.data):  # pylint: disable=protected-access
     result = xl.DataArray(result.data.contiguous(), result.dims, coords)
-  if native:
-    return xl.to_xarray(xl.Dataset({'_': result}))['_']
   return result
 
 

@@ -97,8 +97,7 @@ class EnsembleMetric(m.Metric):
   def compute(self, forecast, truth, region=None, skipna=False):
     """Adds the `ensemble_size` attribute (metrics.py:598-607)."""
     result = super().compute(forecast, truth, region=region, skipna=skipna)
-    return result.assign_attrs(
-        ensemble_size=xl.from_xarray(forecast).sizes[self.ensemble_dim])
+    return result.assign_attrs(ensemble_size=forecast.sizes[self.ensemble_dim])
 
 
 @dataclasses.dataclass
@@ -106,10 +105,9 @@ class CRPSSkill(EnsembleMetric):
   """E|X - Y| (metrics.py:697-715)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     _get_n_ensemble(forecast, self.ensemble_dim)
     res = _ens_request(forecast, truth, self.ensemble_dim, region, skipna)
-    return m._finish(_ens_dataset(res, _mean_stat(_SKILL)), native)  # pylint: disable=protected-access
+    return _ens_dataset(res, _mean_stat(_SKILL))
 
 
 @dataclasses.dataclass
@@ -117,10 +115,9 @@ class CRPSSpread(EnsembleMetric):
   """E|X - X'| (metrics.py:678-694; M < 2 -> zeros, :788-789)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     _get_n_ensemble(forecast, self.ensemble_dim)
     res = _ens_request(forecast, truth, self.ensemble_dim, region, skipna)
-    return m._finish(_ens_dataset(res, _mean_stat(_SPREAD)), native)  # pylint: disable=protected-access
+    return _ens_dataset(res, _mean_stat(_SPREAD))
 
 
 @dataclasses.dataclass
@@ -129,12 +126,11 @@ class CRPS(EnsembleMetric):
   (metrics.py:610-675)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     _get_n_ensemble(forecast, self.ensemble_dim)
     res = _ens_request(forecast, truth, self.ensemble_dim, region, skipna)
     fn = lambda st, mm: (_mean_stat(_SKILL)(st, mm) -
                          0.5 * _mean_stat(_SPREAD)(st, mm))
-    return m._finish(_ens_dataset(res, fn), native)  # pylint: disable=protected-access
+    return _ens_dataset(res, fn)
 
 
 @dataclasses.dataclass
@@ -142,10 +138,9 @@ class EnsembleMeanMSE(EnsembleMetric):
   """MSE of the ensemble mean (metrics.py:1310-1333)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     _get_n_ensemble(forecast, self.ensemble_dim)
     res = _ens_request(forecast, truth, self.ensemble_dim, region, skipna)
-    return m._finish(_ens_dataset(res, _mean_stat(_MSE)), native)  # pylint: disable=protected-access
+    return _ens_dataset(res, _mean_stat(_MSE))
 
 
 @dataclasses.dataclass
@@ -154,12 +149,11 @@ class EnsembleMeanRMSESqrtBeforeTimeAvg(EnsembleMetric):
   (metrics.py:1269-1307)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     _get_n_ensemble(forecast, self.ensemble_dim)
     res = _ens_request(forecast, truth, self.ensemble_dim, region, skipna)
     with np.errstate(invalid='ignore'):
       fn = lambda st, mm: np.sqrt(_mean_stat(_MSE)(st, mm))
-      return m._finish(_ens_dataset(res, fn), native)  # pylint: disable=protected-access
+      return _ens_dataset(res, fn)
 
 
 def _zeros_for_single_member(st, idx):
@@ -173,14 +167,13 @@ class EnsembleVariance(EnsembleMetric):
   """Spatial mean of the ddof=1 ensemble variance (metrics.py:1213-1241)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     n_ensemble = _get_n_ensemble(forecast, self.ensemble_dim)
     res = _ens_request(forecast, truth, self.ensemble_dim, region, skipna)
     if n_ensemble == 1:
       fn = lambda st, mm: _zeros_for_single_member(st, _VAR)
     else:
       fn = _mean_stat(_VAR)
-    return m._finish(_ens_dataset(res, fn), native)  # pylint: disable=protected-access
+    return _ens_dataset(res, fn)
 
 
 @dataclasses.dataclass
@@ -189,7 +182,6 @@ class EnsembleStddevSqrtBeforeTimeAvg(EnsembleMetric):
   and then the L2 norm squares it again (metrics.py:1185-1210)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     n_ensemble = _get_n_ensemble(forecast, self.ensemble_dim)
     res = _ens_request(forecast, truth, self.ensemble_dim, region, skipna)
     if n_ensemble == 1:
@@ -198,7 +190,7 @@ class EnsembleStddevSqrtBeforeTimeAvg(EnsembleMetric):
       def fn(st, mm):
         with np.errstate(invalid='ignore'):
           return np.sqrt(_mean_stat(_VAR)(st, mm))
-    return m._finish(_ens_dataset(res, fn), native)  # pylint: disable=protected-access
+    return _ens_dataset(res, fn)
 
 
 @dataclasses.dataclass
@@ -207,10 +199,9 @@ class DebiasedEnsembleMeanMSE(EnsembleMetric):
   1336-1363).  NaN for a single member, like the reference."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     _get_n_ensemble(forecast, self.ensemble_dim)
     res = _ens_request(forecast, truth, self.ensemble_dim, region, skipna)
-    return m._finish(_ens_dataset(res, _mean_stat(_DEBIASED)), native)  # pylint: disable=protected-access
+    return _ens_dataset(res, _mean_stat(_DEBIASED))
 
 
 # ------------------------------------------------------------------------------
@@ -255,16 +246,14 @@ class EnergyScoreSkill(EnsembleMetric):
   """mean_m sqrt(SA((x_m - t)^2)) (metrics.py:1499-1517)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     _get_n_ensemble(forecast, self.ensemble_dim)
     if _use_k3(forecast, self.ensemble_dim, skipna):
-      return m._finish(_energy_k3(forecast, truth, self.ensemble_dim,  # pylint: disable=protected-access
-                                  region)[0], native)
+      return _energy_k3(forecast, truth, self.ensemble_dim, region)[0]
     res = m._det_request(forecast, truth, region, skipna)  # pylint: disable=protected-access
     with np.errstate(invalid='ignore'):
       l2 = m._dataset_from(  # pylint: disable=protected-access
           res, lambda st: np.sqrt(m._ratio(st[..., 0], st[..., 6])))  # pylint: disable=protected-access
-    return m._finish(_member_mean(l2, self.ensemble_dim, skipna), native)  # pylint: disable=protected-access
+    return _member_mean(l2, self.ensemble_dim, skipna)
 
 
 @dataclasses.dataclass
@@ -273,16 +262,14 @@ class EnergyScoreSpread(EnsembleMetric):
   (metrics.py:1467-1496); zeros for a single member."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     n_ensemble = _get_n_ensemble(forecast, self.ensemble_dim)
     if _use_k3(forecast, self.ensemble_dim, skipna):
-      return m._finish(_energy_k3(forecast, truth, self.ensemble_dim,  # pylint: disable=protected-access
-                                  region)[1], native)
+      return _energy_k3(forecast, truth, self.ensemble_dim, region)[1]
     if n_ensemble == 1:
       res = m._det_request(forecast, m._zero_truth(forecast), region, skipna)  # pylint: disable=protected-access
       zeros = m._dataset_from(  # pylint: disable=protected-access
           res, lambda st: np.zeros(st.shape[:-1], dtype=np.float64))
-      return m._finish(_member_mean(zeros, self.ensemble_dim, skipna), native)  # pylint: disable=protected-access
+      return _member_mean(zeros, self.ensemble_dim, skipna)
     a = self._ensemble_slice(forecast, slice(None, -1))  # views, no copies
     b = self._ensemble_slice(forecast, slice(1, None))
     res = m._det_stats(a, b, None, [region], skipna)  # pylint: disable=protected-access
@@ -291,7 +278,7 @@ class EnergyScoreSpread(EnsembleMetric):
     with np.errstate(invalid='ignore'):
       l2 = m._dataset_from(  # pylint: disable=protected-access
           res, lambda st: np.sqrt(m._ratio(st[..., 0], st[..., 6])))  # pylint: disable=protected-access
-    return m._finish(_member_mean(l2, self.ensemble_dim, skipna), native)  # pylint: disable=protected-access
+    return _member_mean(l2, self.ensemble_dim, skipna)
 
 
 @dataclasses.dataclass
@@ -299,11 +286,10 @@ class EnergyScore(EnsembleMetric):
   """ES = skill - spread / 2 (metrics.py:1402-1464)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    fc, tr, native = m._prep(forecast, truth)  # pylint: disable=protected-access
-    _get_n_ensemble(fc, self.ensemble_dim)
-    if _use_k3(fc, self.ensemble_dim, skipna):
-      skill, spread = _energy_k3(fc, tr, self.ensemble_dim, region)
-      return m._finish(skill - 0.5 * spread, native)  # pylint: disable=protected-access
+    _get_n_ensemble(forecast, self.ensemble_dim)
+    if _use_k3(forecast, self.ensemble_dim, skipna):
+      skill, spread = _energy_k3(forecast, truth, self.ensemble_dim, region)
+      return skill - 0.5 * spread
     return EnergyScoreSkill(self.ensemble_dim).compute_chunk(
         forecast, truth, region=region, skipna=skipna
     ) - 0.5 * EnergyScoreSpread(self.ensemble_dim).compute_chunk(
@@ -357,7 +343,6 @@ class _SpatialEnsembleMetric(EnsembleMetric):
   per-time maps, `compute` fuses the time mean into the kernel."""
 
   def _maps(self, forecast, truth, reduce_dim, skipna):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     n_ensemble = _get_n_ensemble(forecast, self.ensemble_dim)
     ds = _ens_map_request(forecast, truth, self.ensemble_dim, self._BIT,
                           reduce_dim, skipna)
@@ -367,7 +352,7 @@ class _SpatialEnsembleMetric(EnsembleMetric):
         da = ds[name]
         ds[name] = xl.DataArray(xl.zeros_like(da).data, da.dims, da.coords,
                                 name)
-    return m._finish(ds, native)  # pylint: disable=protected-access
+    return ds
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
     del region  # ignored, like the reference
@@ -375,9 +360,8 @@ class _SpatialEnsembleMetric(EnsembleMetric):
 
   def compute(self, forecast, truth, region=None, skipna=False):
     del region
-    fc = xl.from_xarray(forecast)
-    result = self._maps(forecast, truth, m._avg_dim(fc), skipna)  # pylint: disable=protected-access
-    return result.assign_attrs(ensemble_size=fc.sizes[self.ensemble_dim])
+    result = self._maps(forecast, truth, m._avg_dim(forecast), skipna)  # pylint: disable=protected-access
+    return result.assign_attrs(ensemble_size=forecast.sizes[self.ensemble_dim])
 
 
 @dataclasses.dataclass

@@ -52,7 +52,6 @@ class RankHistogram(ens.EnsembleMetric):
     return self.num_bins
 
   def _hist(self, forecast, truth, reduce_dim):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     n_ensemble = ens._get_n_ensemble(forecast, self.ensemble_dim)  # pylint: disable=protected-access
     nbins = self._num_bins_actual(n_ensemble)
     seed = self._seed
@@ -70,7 +69,7 @@ class RankHistogram(ens.EnsembleMetric):
       coords.pop(self.ensemble_dim, None)
       coords['bins'] = xl.Coord(('bins',), np.arange(nbins))
       out[name] = xl.DataArray(hist, tuple(dims) + ('bins',), coords, name)
-    return m._finish(out, native)  # pylint: disable=protected-access
+    return out
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
     del region, skipna  # ignored, like the reference
@@ -78,11 +77,11 @@ class RankHistogram(ens.EnsembleMetric):
 
   def compute(self, forecast, truth, region=None, skipna=False):
     del region, skipna
-    fc = xl.from_xarray(forecast)
-    result = self._hist(forecast, truth, m._avg_dim(fc))  # pylint: disable=protected-access
-    return result.assign_attrs(ensemble_size=fc.sizes[self.ensemble_dim])
+    result = self._hist(forecast, truth, m._avg_dim(forecast))  # pylint: disable=protected-access
+    return result.assign_attrs(ensemble_size=forecast.sizes[self.ensemble_dim])
 
 
+@xl.boundary
 def central_reliability(hist):
   """Reliability diagram for central histogram probabilities
   (weatherbench2/metrics.py:2045-2126), computed on an already reduced rank
@@ -94,11 +93,8 @@ def central_reliability(hist):
   perfectly calibrated forecast would give, `desired_prob` (with the integer
   `prob_index` as a coordinate along it).
   """
-  native = xl.is_native_xarray(hist)
-  ds = xl.from_xarray(hist)
-  single = isinstance(ds, xl.DataArray)
-  if single:
-    ds = xl.Dataset({ds.name or '_': ds})
+  single = isinstance(hist, xl.DataArray)
+  ds = xl.Dataset({hist.name or '_': hist}) if single else hist
   n_bins = ds.sizes['bins']
   if n_bins < 3:
     raise ValueError(f'Too few bins. {n_bins=} but should be >= 3')
@@ -137,7 +133,4 @@ def central_reliability(hist):
     coords['desired_prob'] = xl.Coord(('desired_prob',), desired)
     coords['prob_index'] = xl.Coord(('desired_prob',), np.arange(desired.size))
     out[name] = xl.DataArray(data, dims, coords, name, da.attrs)
-  if single:
-    result = out[list(out.keys())[0]]
-    return xl.to_xarray(xl.Dataset({'_': result}))['_'] if native else result
-  return xl.to_xarray(out) if native else out
+  return out[list(out.keys())[0]] if single else out

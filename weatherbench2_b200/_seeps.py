@@ -68,7 +68,6 @@ class SpatialSEEPS(m.Metric):
     return dry_fraction.mean(('hour', 'dayofyear'))
 
   def _maps(self, forecast, truth, reduce_dim, skipna):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     ctx = m._context()  # pylint: disable=protected-access
     clim = xl.from_xarray(self.climatology)
     name = self.precip_name
@@ -89,19 +88,16 @@ class SpatialSEEPS(m.Metric):
         self.min_p1, self.max_p1, reduce_dim, skipna)
     out = xl.Dataset()
     out[name] = xl.DataArray(maps, dims, m._map_coords(dims, f_da, t_da), name)  # pylint: disable=protected-access
-    return out, native
+    return out
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
     del region, skipna  # ignored (metrics.py:470): the p1 mask forces NaNs
-    out, native = self._maps(forecast, truth, None, False)
-    return m._finish(out, native)  # pylint: disable=protected-access
+    return self._maps(forecast, truth, None, False)
 
   def compute(self, forecast, truth, region=None, skipna=False):
     """metrics.py:117-138 with the time mean fused into the kernel."""
     del region
-    out, native = self._maps(forecast, truth,
-                             m._avg_dim(xl.from_xarray(forecast)), skipna)  # pylint: disable=protected-access
-    return m._finish(out, native)  # pylint: disable=protected-access
+    return self._maps(forecast, truth, m._avg_dim(forecast), skipna)  # pylint: disable=protected-access
 
 
 @dataclasses.dataclass
@@ -114,11 +110,10 @@ class SEEPS(SpatialSEEPS):
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
     del skipna  # effectively True because of the p1 mask (metrics.py:526)
-    out, native = self._maps(forecast, truth, None, False)
-    return m._finish(m._spatial_average(out, region=region, skipna=True),  # pylint: disable=protected-access
-                     native)
+    out = self._maps(forecast, truth, None, False)
+    return m._spatial_average(out, region=region, skipna=True)  # pylint: disable=protected-access
 
   def compute(self, forecast, truth, region=None, skipna=False):
-    avg_dim = m._avg_dim(xl.from_xarray(forecast))  # pylint: disable=protected-access
+    avg_dim = m._avg_dim(forecast)  # pylint: disable=protected-access
     return self.compute_chunk(forecast, truth, region=region,
                               skipna=skipna).mean(avg_dim, skipna=skipna)

@@ -116,9 +116,8 @@ class GaussianCRPS(m.Metric):
   """The analytical CRPS of a Gaussian forecast (metrics.py:849-899)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     res = _gaussian_request(forecast, truth, None, region, skipna)
-    return m._finish(_stats_to_dataset(res, _GCRPS, None, False, {}), native)  # pylint: disable=protected-access
+    return _stats_to_dataset(res, _GCRPS, None, False, {})
 
 
 @dataclasses.dataclass
@@ -126,9 +125,8 @@ class GaussianVariance(m.Metric):
   """The variance of a Gaussian forecast (metrics.py:902-928)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     res = _gaussian_request(forecast, truth, None, region, skipna)
-    return m._finish(_stats_to_dataset(res, _GVAR, None, False, {}), native)  # pylint: disable=protected-access
+    return _stats_to_dataset(res, _GVAR, None, False, {})
 
 
 @dataclasses.dataclass
@@ -149,12 +147,11 @@ class _GaussianThresholdMetric(ThresholdMetric):
   _SUM = False
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     res = _gaussian_request(forecast, truth, list(self.thresholds), region,
                             skipna)
     ds = _stats_to_dataset(res, self._SLOT, _quantile_coords(self.thresholds),
                            self._SUM, self._attrs())
-    return m._finish(ds, native)  # pylint: disable=protected-access
+    return ds
 
 
 @dataclasses.dataclass
@@ -225,13 +222,12 @@ class _EnsembleThresholdMetric(ens.EnsembleMetric, ThresholdMetric):
   _SUM = False
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     ens._get_n_ensemble(forecast, self.ensemble_dim)  # pylint: disable=protected-access
     res = _ens_threshold_request(forecast, truth, self.ensemble_dim,
                                  list(self.thresholds), region, skipna)
     ds = _stats_to_dataset(res, self._SLOT, _quantile_coords(self.thresholds),
                            self._SUM, self._attrs())
-    return m._finish(ds, native)  # pylint: disable=protected-access
+    return ds
 
 
 @dataclasses.dataclass
@@ -282,7 +278,6 @@ class _SpatialEnsembleThresholdMetric(_EnsembleThresholdMetric):
   pass.  `region` is ignored like in the reference (spatial_agg=False)."""
 
   def _maps(self, forecast, truth, reduce_dim, skipna):
-    forecast, truth, native = m._prep(forecast, truth)  # pylint: disable=protected-access
     ens._get_n_ensemble(forecast, self.ensemble_dim)  # pylint: disable=protected-access
     ctx = m._context()  # pylint: disable=protected-access
     thresholds = list(self.thresholds)
@@ -305,7 +300,7 @@ class _SpatialEnsembleThresholdMetric(_EnsembleThresholdMetric):
         coords['quantile'] = _quantile_coords(thresholds)
         out[name] = xl.DataArray(maps, ('quantile',) + tuple(dims), coords,
                                  name)
-    return m._finish(out, native)  # pylint: disable=protected-access
+    return out
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
     del region
@@ -313,9 +308,8 @@ class _SpatialEnsembleThresholdMetric(_EnsembleThresholdMetric):
 
   def compute(self, forecast, truth, region=None, skipna=False):
     del region
-    fc = xl.from_xarray(forecast)
-    result = self._maps(forecast, truth, m._avg_dim(fc), skipna)  # pylint: disable=protected-access
-    return result.assign_attrs(ensemble_size=fc.sizes[self.ensemble_dim])
+    result = self._maps(forecast, truth, m._avg_dim(forecast), skipna)  # pylint: disable=protected-access
+    return result.assign_attrs(ensemble_size=forecast.sizes[self.ensemble_dim])
 
 
 @dataclasses.dataclass

@@ -28,8 +28,10 @@ EARTH_RADIUS_M = 1000 * (6357 + 6378) / 2  # weatherbench2/schema.py:59
 
 
 @dataclasses.dataclass
-class DerivedVariable:
+class DerivedVariable(xl.Boundary):
   """Derived variable base class (derived_variables.py:28-56)."""
+
+  _boundary_methods = ('compute', 'compute_latitude_mean')
 
   @property
   def base_variables(self) -> list[str]:
@@ -93,12 +95,10 @@ class ZonalEnergySpectrum(DerivedVariable):
     scripts/compute_zonal_energy_spectrum.py:234, is sum / count); the
     dimension is dropped from the result.
     """
-    native = xl.is_native_xarray(dataset)
-    ds = xl.from_xarray(dataset)
-    spacing = self.lon_spacing_m(ds).values
-    da = ds[self.variable_name]
-    lat = ds['latitude'].values
-    lon = ds['longitude'].values
+    spacing = self.lon_spacing_m(dataset).values
+    da = dataset[self.variable_name]
+    lat = dataset['latitude'].values
+    lon = dataset['longitude'].values
     if 'latitude' not in da.dims or 'longitude' not in da.dims:
       raise ValueError(f'{self.variable_name} needs latitude and longitude')
     outer = tuple(d for d in da.dims if d not in ('latitude', 'longitude'))
@@ -157,7 +157,7 @@ class ZonalEnergySpectrum(DerivedVariable):
     result = xl.DataArray(values, dims, coords, self.variable_name)
     if not is_torch:
       result = result.transpose(*ref_dims)
-    return xl.to_xarray(result) if native else result
+    return result
 
 
   def compute_latitude_mean(self, dataset, time_mean_dim: t.Optional[str] = None,
@@ -172,12 +172,10 @@ class ZonalEnergySpectrum(DerivedVariable):
     `zonal_wavenumber`; no frequency / wavelength coordinates (they depend on
     latitude)."""
     from weatherbench2_b200 import _spatial as sp  # pylint: disable=import-outside-toplevel
-    native = xl.is_native_xarray(dataset)
-    ds = xl.from_xarray(dataset)
-    self.lon_spacing_m(ds)  # uniform-longitude check (derived_variables.py:583-590)
-    da = ds[self.variable_name]
-    lat = ds['latitude'].values
-    lon = ds['longitude'].values
+    self.lon_spacing_m(dataset)  # uniform-longitude check (derived_variables.py:583-590)
+    da = dataset[self.variable_name]
+    lat = dataset['latitude'].values
+    lon = dataset['longitude'].values
     outer = tuple(d for d in da.dims if d not in ('latitude', 'longitude'))
     if time_mean_dim is not None:
       if time_mean_dim not in outer:
@@ -218,10 +216,10 @@ class ZonalEnergySpectrum(DerivedVariable):
     coords = {k: c for k, c in work.coords.items()
               if all(d in out_outer for d in c.dims)}
     coords['zonal_wavenumber'] = xl.Coord(('zonal_wavenumber',), np.arange(nk))
-    result = xl.DataArray(values, dims, coords, self.variable_name)
-    return xl.to_xarray(result) if native else result
+    return xl.DataArray(values, dims, coords, self.variable_name)
 
 
+@xl.boundary
 def interpolate_spectral_frequencies(spectrum, wavenumber_dim: str,
                                      frequencies=None, method: str = 'linear'):
   """Interpolate the frequencies of `spectrum` (as produced by
@@ -233,9 +231,7 @@ def interpolate_spectral_frequencies(spectrum, wavenumber_dim: str,
   (:658-664).  Linear interpolation only (the kernel is a gather + lerp)."""
   if method != 'linear':
     raise NotImplementedError('only method="linear" runs on the device')
-  native = xl.is_native_xarray(spectrum)
-  sp_ = xl.from_xarray(spectrum)
-  freq = sp_.coords['frequency']
+  freq = spectrum.coords['frequency']
   if set(freq.dims) != {wavenumber_dim, 'latitude'}:
     raise ValueError(f'{freq.dims=} was not a permutation of '
                      f'("{wavenumber_dim}", "latitude")')
@@ -253,8 +249,9 @@ def interpolate_spectral_frequencies(spectrum, wavenumber_dim: str,
   table = np.ascontiguousarray(fv.T)  # (latitude, wavenumber), increasing in k
   if nk < 2 or not (np.diff(table, axis=1) > 0).all():
     raise ValueError('the frequency coordinate must increase with wavenumber')
-  outer = tuple(d for d in sp_.dims if d not in ('latitude', wavenumber_dim))
-  work = sp_.transpose(*(outer + ('latitude', wavenumber_dim)))
+  outer = tuple(d for d in spectrum.dims
+                if d not in ('latitude', wavenumber_dim))
+  work = spectrum.transpose(*(outer + ('latitude', wavenumber_dim)))
   data = work.data
   oshape = tuple(work.sizes[d] for d in outer)
   nfield = int(np.prod(oshape)) if oshape else 1
@@ -274,13 +271,14 @@ def interpolate_spectral_frequencies(spectrum, wavenumber_dim: str,
     # "Interp didn't deal well with the infinite wavelength, so just reset"
     coords['wavelength'] = xl.Coord(('frequency',), 1 / frequencies,
                                     {'units': 'm'})
-  result = xl.DataArray(values, dims, coords, sp_.name, sp_.attrs)
+  result = xl.DataArray(values, dims, coords, spectrum.name, spectrum.attrs)
   # the reference's groupby('latitude').apply keeps latitude where it was and
   # puts frequency in the wavenumber's place
-  ref_dims = tuple('frequency' if d == wavenumber_dim else d for d in sp_.dims)
+  ref_dims = tuple('frequency' if d == wavenumber_dim else d
+                   for d in spectrum.dims)
   if not xl._is_torch(values):  # pylint: disable=protected-access
     result = result.transpose(*ref_dims)
-  return xl.to_xarray(result) if native else result
+  return result
 
 
 # Wind variables live in _derived_wind.py (they need DerivedVariable).

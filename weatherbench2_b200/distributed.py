@@ -238,7 +238,7 @@ def evaluate_sharded(forecast: xl.Dataset, truth: xl.Dataset, eval_config,
       if temporal_mean:
         acc.add(res)
       else:
-        per_chunk.append(xl.from_xarray(res))
+        per_chunk.append(res)
   if not temporal_mean:
     return _gather_chunks(per_chunk, mine, chunk_dim, world, group, device)
   if not acc.sums:

@@ -86,14 +86,12 @@ def select_truth_at_valid_time(truth: xl.Dataset, forecast: xl.Dataset
 LazyGather = xl.LazyGather  # defined next to the container it extends
 
 
+@xl.boundary
 def _metric_and_region_loop(forecast: xl.Dataset, truth: xl.Dataset,
                             eval_config: config.Eval, skipna: bool,
                             compute_chunk: bool = False) -> xl.Dataset:
   """Metric results looping over metrics and regions (evaluation.py:388-438).
   Result variables have dims (metric, [region], ...)."""
-  native = xl.is_native_xarray(forecast)
-  forecast = xl.from_xarray(forecast)
-  truth = xl.from_xarray(truth)
   logging.info('Starting _metric_and_region_loop')
   for name, dv in eval_config.derived_variables.items():
     forecast[name] = dv.compute(forecast)
@@ -118,19 +116,18 @@ def _metric_and_region_loop(forecast: xl.Dataset, truth: xl.Dataset,
       if eval_config.regions is not None:
         tmp_results = []
         for region_name, region in eval_config.regions.items():
-          tmp = xl.from_xarray(eval_fn(forecast=forecast, truth=truth,
-                                       region=region, skipna=skipna))
+          tmp = eval_fn(forecast=forecast, truth=truth, region=region,
+                        skipna=skipna)
           tmp_results.append(tmp.expand_dims(
               {'metric': np.array([name], dtype=object),
                'region': np.array([region_name], dtype=object)}))
         result = xl.concat(tmp_results, 'region')
       else:
-        result = xl.from_xarray(eval_fn(
-            forecast=forecast, truth=truth, skipna=skipna)).expand_dims(
-                {'metric': np.array([name], dtype=object)})
+        result = eval_fn(forecast=forecast, truth=truth,
+                         skipna=skipna).expand_dims(
+                             {'metric': np.array([name], dtype=object)})
       results.append(result)
-  merged = xl.merge(results)
-  return xl.to_xarray(merged) if native else merged
+  return xl.merge(results)
 
 
 def _ensure_nonempty(dataset: xl.Dataset, message: str = '') -> None:

@@ -35,10 +35,10 @@ REALIZATION = 'realization'
 LAT, LON = sp.LAT, sp.LON
 
 
+@xl.boundary
 def get_lat_weights(ds) -> xl.DataArray:
   """Latitude/area weights from the dataset's latitude coordinate
   (weatherbench2/metrics.py:55-60)."""
-  ds = xl.from_xarray(ds)
   lat = ds['latitude'].values if 'latitude' in ds else ds.latitude.values
   w = sp.lat_weights(lat)
   return xl.DataArray(w, ('latitude',), {'latitude': lat})
@@ -271,21 +271,14 @@ def _dataset_from(results: dict, fn) -> xl.Dataset:
   return out
 
 
-def _prep(forecast, truth):
-  native = xl.is_native_xarray(forecast)
-  return xl.from_xarray(forecast), xl.from_xarray(truth), native
-
-
-def _finish(ds: xl.Dataset, native: bool):
-  return xl.to_xarray(ds) if native else ds
-
-
 # ------------------------------------------------------------------------------
 # Metric classes
 # ------------------------------------------------------------------------------
 @dataclasses.dataclass
-class Metric:
+class Metric(xl.Boundary):
   """Base class for metrics (weatherbench2/metrics.py:84-138)."""
+
+  _boundary_methods = ('compute', 'compute_chunk')
 
   def compute_chunk(self, forecast, truth, region: t.Optional[Region] = None,
                     skipna: bool = False):
@@ -324,23 +317,22 @@ def _zero_truth(ds: xl.Dataset) -> xl.Dataset:
   return zeros
 
 
+@xl.boundary
 def _spatial_average(dataset, region: t.Optional[Region], skipna: bool):
   """Weighted spatial mean of an arbitrary (lat, lon) dataset
   (weatherbench2/metrics.py:141-163), evaluated on the GPU as the Bias
   statistic of (dataset - 0)."""
-  ds, _, native = _prep(dataset, dataset)
-  res = _det_stats(ds, _zero_truth(ds), None, [region], skipna)
-  return _finish(_dataset_from(
-      res, lambda st: _ratio(st[..., 0, 2], st[..., 0, 6])), native)
+  res = _det_stats(dataset, _zero_truth(dataset), None, [region], skipna)
+  return _dataset_from(res, lambda st: _ratio(st[..., 0, 2], st[..., 0, 6]))
 
 
+@xl.boundary
 def _spatial_average_l2_norm(dataset, region, skipna):
   """sqrt(spatial_average(ds**2)) (metrics.py:166-172)."""
-  ds, _, native = _prep(dataset, dataset)
-  res = _det_stats(ds, _zero_truth(ds), None, [region], skipna)
+  res = _det_stats(dataset, _zero_truth(dataset), None, [region], skipna)
   with np.errstate(invalid='ignore'):
-    return _finish(_dataset_from(
-        res, lambda st: np.sqrt(_ratio(st[..., 0, 0], st[..., 0, 6]))), native)
+    return _dataset_from(
+        res, lambda st: np.sqrt(_ratio(st[..., 0, 0], st[..., 0, 6])))
 
 
 def _wind_vector_stat(forecast, truth, u_name, v_name, region, skipna):
@@ -390,10 +382,8 @@ class WindVectorMSE(Metric):
   vector_name: str
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = _prep(forecast, truth)
-    da = _wind_vector_stat(forecast, truth, self.u_name, self.v_name, region,
-                           skipna)
-    return xl.to_xarray(da) if native else da
+    return _wind_vector_stat(forecast, truth, self.u_name, self.v_name, region,
+                             skipna)
 
 
 @dataclasses.dataclass
@@ -419,16 +409,15 @@ class RMSESqrtBeforeTimeAvg(Metric):
   wind_vector_rmse: t.Optional[list] = None
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = _prep(forecast, truth)
     res = _det_request(forecast, truth, region, skipna)
     with np.errstate(invalid='ignore'):
       results = _dataset_from(
           res, lambda st: np.sqrt(_ratio(st[..., 0], st[..., 6])))
     if self.wind_vector_rmse is not None:
       for wv in self.wind_vector_rmse:
-        results[wv.vector_name] = xl.from_xarray(wv.compute_chunk(
-            forecast, truth, region=region, skipna=skipna))
-    return _finish(results, native)
+        results[wv.vector_name] = wv.compute_chunk(
+            forecast, truth, region=region, skipna=skipna)
+    return results
 
 
 @dataclasses.dataclass
@@ -438,14 +427,13 @@ class MSE(Metric):
   wind_vector_mse: t.Optional[list] = None
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = _prep(forecast, truth)
     res = _det_request(forecast, truth, region, skipna)
     results = _dataset_from(res, lambda st: _ratio(st[..., 0], st[..., 6]))
     if self.wind_vector_mse is not None:
       for wv in self.wind_vector_mse:
-        results[wv.vector_name] = xl.from_xarray(wv.compute_chunk(
-            forecast, truth, region=region, skipna=skipna))
-    return _finish(results, native)
+        results[wv.vector_name] = wv.compute_chunk(
+            forecast, truth, region=region, skipna=skipna)
+    return results
 
 
 @dataclasses.dataclass
@@ -453,10 +441,8 @@ class MAE(Metric):
   """Mean absolute error (metrics.py:319-330)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = _prep(forecast, truth)
     res = _det_request(forecast, truth, region, skipna)
-    return _finish(_dataset_from(
-        res, lambda st: _ratio(st[..., 1], st[..., 6])), native)
+    return _dataset_from(res, lambda st: _ratio(st[..., 1], st[..., 6]))
 
 
 @dataclasses.dataclass
@@ -464,10 +450,8 @@ class Bias(Metric):
   """Bias (metrics.py:348-359)."""
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = _prep(forecast, truth)
     res = _det_request(forecast, truth, region, skipna)
-    return _finish(_dataset_from(
-        res, lambda st: _ratio(st[..., 2], st[..., 6])), native)
+    return _dataset_from(res, lambda st: _ratio(st[..., 2], st[..., 6]))
 
 
 def _map_coords(out_dims, *sources: xl.DataArray) -> dict:
@@ -496,14 +480,13 @@ class _SpatialDetMetric(Metric):
   never materialised.  `region` is ignored like in the reference."""
 
   def _maps(self, forecast, truth, reduce_dim, skipna):
-    forecast, truth, native = _prep(forecast, truth)
     ctx = _context()
     out = xl.Dataset()
     for name, f_da, t_da, f_op, t_op in _paired_operands(forecast, truth):
       maps, dims = sp.run_det_maps(ctx, f_op, t_op, self._STAT, reduce_dim,
                                    skipna)
       out[name] = xl.DataArray(maps, dims, _map_coords(dims, f_da, t_da), name)
-    return _finish(out, native)
+    return out
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
     del region, skipna  # ignored (metrics.py:315, 344, 373)
@@ -543,7 +526,6 @@ class ACC(Metric):
     return id(self)
 
   def compute_chunk(self, forecast, truth, region=None, skipna=False):
-    forecast, truth, native = _prep(forecast, truth)
     clim = xl.from_xarray(self.climatology)
     # fail like the reference when variables are missing (metrics.py:73-77)
     _get_climatology_chunk(clim, truth)
@@ -556,7 +538,7 @@ class ACC(Metric):
       with np.errstate(invalid='ignore', divide='ignore'):
         return cov / np.sqrt(ff * tt)
 
-    return _finish(_dataset_from(res, acc), native)
+    return _dataset_from(res, acc)
 
 
 # Ensemble metrics live in _ensemble.py (they need the helpers above).

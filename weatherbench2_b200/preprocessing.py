@@ -24,6 +24,7 @@ QUANTILE = 'quantile'
 QUANTILE_STREAM_BUDGET_BYTES = 1 << 30
 
 
+@xl.boundary
 def compute_ensemble_mean(dataset, realization_name: str = REALIZATION,
                           skipna: bool = False):
   """Mean over `realization_name` of every variable that has it
@@ -34,12 +35,10 @@ def compute_ensemble_mean(dataset, realization_name: str = REALIZATION,
   variables are uploaded, reduced and the (M times smaller) mean comes back.
   Variables without the dimension pass through.
   """
-  native = xl.is_native_xarray(dataset)
-  ds = xl.from_xarray(dataset)
   ctx = _lib.default_context()
-  out = xl.Dataset(attrs=ds.attrs)
-  for name in ds.keys():
-    v = ds[name]
+  out = xl.Dataset(attrs=dataset.attrs)
+  for name in dataset.keys():
+    v = dataset[name]
     if realization_name not in v.dims:
       out[name] = v
       continue
@@ -60,7 +59,7 @@ def compute_ensemble_mean(dataset, realization_name: str = REALIZATION,
         lambda i, o: ctx.ens_mean(i[0], m, cells, off, slab, skipna, o[0]),
         dtype=np.float32)
     out[name] = xl.DataArray(values, dims, coords, name, v.attrs)
-  return xl.to_xarray(out) if native else out
+  return out
 
 
 def _check_quantiles(quantiles) -> list:
@@ -106,6 +105,7 @@ def _variable_quantiles(v: xl.DataArray, reduce: list, quantiles: list,
                        perm=perm)[0]
 
 
+@xl.boundary
 def compute_quantiles_core(chunk, quantiles: Sequence[float], dim, *,
                            skipna: bool = False, name_suffix: str = ''):
   """`_evaluate_chunk_core` of scripts/compute_quantiles.py:168-183:
@@ -121,25 +121,23 @@ def compute_quantiles_core(chunk, quantiles: Sequence[float], dim, *,
   through the device in bands and give NumPy.  Reduced dims need not be
   adjacent: when they are not, the variable is copied once, transposed with
   the reduced dims in front (torch on the device, NumPy on the host)."""
-  native = xl.is_native_xarray(chunk)
-  ds = xl.from_xarray(chunk)
   dims = [dim] if isinstance(dim, str) else list(dim)
-  preserve_dims = set(d for d in ds.dims if d not in dims)
-  if not preserve_dims.issubset(set(ds.dims)):
+  preserve_dims = set(d for d in chunk.dims if d not in dims)
+  if not preserve_dims.issubset(set(chunk.dims)):
     raise ValueError(
         f'User specified dim={dims}, which results in preserved dims'
-        f' {preserve_dims} , not being a subset of {set(ds.dims)=}')
+        f' {preserve_dims} , not being a subset of {set(chunk.dims)=}')
   quantiles = _check_quantiles(quantiles)
-  missing = [d for d in dims if d not in ds.dims]
+  missing = [d for d in dims if d not in chunk.dims]
   if missing:
     raise ValueError(f'Dimensions {tuple(missing)} not found in data '
-                     f'dimensions {tuple(ds.dims)}')
-  coords = {k: c for k, c in ds.coords.items()
+                     f'dimensions {tuple(chunk.dims)}')
+  coords = {k: c for k, c in chunk.coords.items()
             if not any(d in dims for d in c.dims)}
   coords[QUANTILE] = xl.Coord((QUANTILE,), np.asarray(quantiles, np.float64))
   out = xl.Dataset(coords=coords)
-  for name in ds.keys():
-    v = ds[name]
+  for name in chunk.keys():
+    v = chunk[name]
     reduce = [d for d in v.dims if d in dims]
     if not reduce and v.dims:
       out[name + name_suffix] = xl.DataArray(v.data, v.dims, attrs=v.attrs)
@@ -147,9 +145,10 @@ def compute_quantiles_core(chunk, quantiles: Sequence[float], dim, *,
     values = _variable_quantiles(v, reduce, quantiles, skipna)
     out[name + name_suffix] = xl.DataArray(
         values, (QUANTILE,) + tuple(d for d in v.dims if d not in reduce))
-  return xl.to_xarray(out) if native else out
+  return out
 
 
+@xl.boundary
 def compute_quantiles(ds, quantiles: Sequence[float], dim, *,
                       skipna: bool = False, name_suffix: str = '',
                       variables: Optional[Sequence[str]] = None,
@@ -162,12 +161,10 @@ def compute_quantiles(ds, quantiles: Sequence[float], dim, *,
   `time_dim` with both ends inclusive and the script's default range, then
   `levels` on `level`, each only where the dim exists), then
   `compute_quantiles_core`."""
-  native = xl.is_native_xarray(ds)
-  ds = _impose_data_selection(xl.from_xarray(ds), variables, levels, time_dim,
-                              time_start, time_stop)
-  out = compute_quantiles_core(ds, quantiles, dim, skipna=skipna,
-                               name_suffix=name_suffix)
-  return xl.to_xarray(out) if native else out
+  ds = _impose_data_selection(ds, variables, levels, time_dim, time_start,
+                              time_stop)
+  return compute_quantiles_core(ds, quantiles, dim, skipna=skipna,
+                                name_suffix=name_suffix)
 
 
 def _impose_data_selection(ds: xl.Dataset, variables, levels, time_dim,
@@ -271,6 +268,7 @@ def _kept_coords(ds: xl.Dataset, dims) -> dict:
           if not any(d in dims for d in c.dims)}
 
 
+@xl.boundary
 def compute_averages(ds, averaging_dims: Sequence[str], *,
                      skipna: bool = False,
                      variables: Optional[Sequence[str]] = None,
@@ -292,9 +290,8 @@ def compute_averages(ds, averaging_dims: Sequence[str], *,
   dims raises ValueError.  CUDA-tensor variables give CUDA tensors; NumPy or
   memmap variables are streamed through the device and give NumPy.  Sums are
   float64 in the order include/wb2b200.h fixes (DESIGN.md section 8g)."""
-  native = xl.is_native_xarray(ds)
-  ds = _impose_data_selection(xl.from_xarray(ds), variables, levels, time_dim,
-                              time_start, time_stop)
+  ds = _impose_data_selection(ds, variables, levels, time_dim, time_start,
+                              time_stop)
   dims = [averaging_dims] if isinstance(averaging_dims, str) else list(
       averaging_dims)
   weights = None
@@ -310,7 +307,7 @@ def compute_averages(ds, averaging_dims: Sequence[str], *,
                             weights=weights)
     out[name] = xl.DataArray(res['mean'],
                              tuple(d for d in v.dims if d not in dims))
-  return xl.to_xarray(out) if native else out
+  return out
 
 
 def _moment_stat(order: str) -> str:
@@ -320,6 +317,7 @@ def _moment_stat(order: str) -> str:
     raise NotImplementedError(f'Order {order} not implemented.') from None
 
 
+@xl.boundary
 def moment_reduce(obs, order: str = 'first',
                   reduce_dims: Sequence[str] = ('longitude', 'latitude'),
                   sel_kwargs: Optional[dict] = None):
@@ -329,22 +327,21 @@ def moment_reduce(obs, order: str = 'first',
   fraction of non-NaN samples, float64).  Unweighted and NaN-skipping, as
   xarray's mean of float data is; other orders raise NotImplementedError."""
   stat = _moment_stat(order)
-  native = xl.is_native_xarray(obs)
-  ds = xl.from_xarray(obs)
   if sel_kwargs:
-    ds = ds.sel(sel_kwargs)
+    obs = obs.sel(sel_kwargs)
   dims = [reduce_dims] if isinstance(reduce_dims, str) else list(reduce_dims)
-  for name in ds.keys():
-    _check_average(ds[name], dims)
-  out = xl.Dataset(coords=_kept_coords(ds, dims))
-  for name in ds.keys():
-    v = ds[name]
+  for name in obs.keys():
+    _check_average(obs[name], dims)
+  out = xl.Dataset(coords=_kept_coords(obs, dims))
+  for name in obs.keys():
+    v = obs[name]
     res = _variable_average(v, dims, (stat,), skipna=True)
     out[name] = xl.DataArray(res[stat],
                              tuple(d for d in v.dims if d not in dims))
-  return xl.to_xarray(out) if native else out
+  return out
 
 
+@xl.boundary
 def compute_statistical_moments(obs, *, start_year: Optional[int] = 1990,
                                 end_year: Optional[int] = 2020,
                                 time_dim: str = 'time'):
@@ -358,20 +355,18 @@ def compute_statistical_moments(obs, *, start_year: Optional[int] = 1990,
   steps.  The result has variables `{var}_{order}`, order-major as the
   script's template, with dims ('moment', *rest): `moment` has size 1 and no
   coordinate."""
-  native = xl.is_native_xarray(obs)
-  ds = xl.from_xarray(obs)
   if start_year is not None and end_year is not None:
-    index = pd.Index(ds.coords[time_dim].values)
-    ds = ds.isel({time_dim: index.slice_indexer(str(start_year),
-                                                str(end_year))})
+    index = pd.Index(obs.coords[time_dim].values)
+    obs = obs.isel({time_dim: index.slice_indexer(str(start_year),
+                                                  str(end_year))})
   space = ['longitude', 'latitude']
   gone = space + [time_dim]
-  out = xl.Dataset(coords=_kept_coords(ds, gone))
-  for name in ds.keys():
-    _check_average(ds[name], gone)
+  out = xl.Dataset(coords=_kept_coords(obs, gone))
+  for name in obs.keys():
+    _check_average(obs[name], gone)
   results = {}
-  for name in ds.keys():
-    v = ds[name]
+  for name in obs.keys():
+    v = obs[name]
     spatial = _variable_average(v, space, _STATS, skipna=True)
     sdims = tuple(d for d in v.dims if d not in space)
     rest = tuple(d for d in sdims if d != time_dim)
@@ -380,7 +375,7 @@ def compute_statistical_moments(obs, *, start_year: Optional[int] = 1990,
       m = _variable_average(s, [time_dim], ('mean',), skipna=True)['mean']
       results[(order, name)] = (m.reshape((1,) + tuple(m.shape)), rest)
   for order in MOMENT_ORDERS:
-    for name in ds.keys():
+    for name in obs.keys():
       values, rest = results[(order, name)]
       out[f'{name}_{order}'] = xl.DataArray(values, (MOMENT,) + rest)
-  return xl.to_xarray(out) if native else out
+  return out

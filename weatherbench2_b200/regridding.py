@@ -262,17 +262,16 @@ class Regridder:
     del ctx, src_ptr, dst_ptr, nfield
     return False
 
+  @xl.boundary
   def regrid_dataset(self, dataset):
     """Regrid a Dataset from source to target (regridding.py:193-209)."""
-    native = xl.is_native_xarray(dataset)
-    ds = xl.from_xarray(dataset)
-    lat = ds['latitude'].values
+    lat = dataset['latitude'].values
     if not (np.diff(lat) > 0).all():
-      ds = ds.isel(latitude=np.arange(lat.size)[::-1])
-    assert (np.diff(ds['latitude'].values) > 0).all()
-    out = xl.Dataset(attrs=ds.attrs)
-    for name in ds.keys():
-      v = ds[name]
+      dataset = dataset.isel(latitude=np.arange(lat.size)[::-1])
+    assert (np.diff(dataset['latitude'].values) > 0).all()
+    out = xl.Dataset(attrs=dataset.attrs)
+    for name in dataset.keys():
+      v = dataset[name]
       if 'longitude' not in v.dims or 'latitude' not in v.dims:
         out[name] = v
         continue
@@ -288,7 +287,7 @@ class Regridder:
                                     np.asarray(self.target.latitudes))
       out[name] = xl.DataArray(arr, core_last, coords, name,
                                v.attrs).transpose(*dims)
-    return xl.to_xarray(out) if native else out
+    return out
 
 
 class ConservativeRegridder(Regridder):

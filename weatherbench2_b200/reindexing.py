@@ -68,10 +68,6 @@ REFLECT_RANGE = 'REFLECT_RANGE'
 ONE_DAY = pd.Timedelta('1D')
 
 
-def _public(obj, result):
-  return xl.to_xarray(result) if xl.is_native_xarray(obj) else result
-
-
 def _source_dtype(da: xl.DataArray, allow_int: bool) -> np.dtype:
   """The dtype the gather reads `da` in: its own float32 / float64, or
   float64 for integers when `allow_int`."""
@@ -154,6 +150,7 @@ def _variables(ds, variables):
 
 
 # ---- expand_climatology ---------------------------------------------------------
+@xl.boundary
 def expand_climatology(climatology, *, time_start: str = '2017-01-01',
                        time_stop: str = '2017-12-31',
                        variables: Optional[Sequence[str]] = None):
@@ -162,9 +159,8 @@ def expand_climatology(climatology, *, time_start: str = '2017-01-01',
   `pd.date_range(time_start, time_stop, freq=hour_delta h)`, where hour_delta
   is hour[1] - hour[0], or 24 without an `hour` coordinate.  Output dims are
   (time, *other dims in source order); dayofyear and hour are dropped."""
-  ds = xl.from_xarray(climatology)
-  if 'hour' in ds.coords:
-    hours = np.asarray(ds.coords['hour'].values)
+  if 'hour' in climatology.coords:
+    hours = np.asarray(climatology.coords['hour'].values)
     if hours.size < 2:
       raise ValueError('a climatology with an hour coordinate needs at least '
                        f'two hours to give the time step; it has {hours}')
@@ -175,15 +171,16 @@ def expand_climatology(climatology, *, time_start: str = '2017-01-01',
     time_dims = ('dayofyear',)
   times = pd.date_range(time_start, time_stop,
                         freq=hour_delta * pd.Timedelta('1h')).as_unit('ns')
-  maps = {'dayofyear': ((TIME,), _positions(ds.coords['dayofyear'].values,
-                                            times.dayofyear.values, 'dayofyear'))}
+  doy = climatology.coords['dayofyear'].values
+  maps = {'dayofyear': ((TIME,), _positions(doy, times.dayofyear.values,
+                                            'dayofyear'))}
   if 'hour' in time_dims:
     maps['hour'] = ((TIME,), _positions(hours, times.hour.values, 'hour'))
-  coords = _other_coords(ds, time_dims)
+  coords = _other_coords(climatology, time_dims)
   coords[TIME] = xl.Coord((TIME,), times.values)
-  out = xl.Dataset(coords=coords, attrs=ds.attrs)
-  for name in _variables(ds, variables):
-    da = ds[name]
+  out = xl.Dataset(coords=coords, attrs=climatology.attrs)
+  for name in _variables(climatology, variables):
+    da = climatology[name]
     lacking = [d for d in time_dims if d not in da.dims]
     if lacking:
       raise ValueError(f'variable {name!r} has no {lacking} dims to expand '
@@ -192,7 +189,7 @@ def expand_climatology(climatology, *, time_start: str = '2017-01-01',
     sizes = dict(da.sizes, **{TIME: times.size})
     data = _gather(da, dims, sizes, maps, _source_dtype(da, False))
     out[name] = xl.DataArray(data, dims, name=name, attrs=da.attrs)
-  return _public(climatology, out)
+  return out
 
 
 # ---- index_on_valid_time --------------------------------------------------------
@@ -237,6 +234,7 @@ def _common_axis(ds, dim: str) -> int:
   return next(iter(axes.values()))
 
 
+@xl.boundary
 def index_on_valid_time(forecast, *,
                         desired_time_dims: str = VALID_AND_DELTA):
   """scripts/index_on_valid_time.py without Beam or zarr.  A
@@ -248,12 +246,11 @@ def index_on_valid_time(forecast, *,
   becomes `init` and valid `time` takes the lead axis's position."""
   if desired_time_dims not in (VALID_AND_DELTA, VALID_AND_INIT):
     raise ValueError(f'Unhandled desired_time_dims={desired_time_dims!r}')
-  ds = xl.from_xarray(forecast)
-  init = np.asarray(ds.coords[TIME].values)
-  leads = np.asarray(ds.coords[DELTA].values)
+  init = np.asarray(forecast.coords[TIME].values)
+  leads = np.asarray(forecast.coords[DELTA].values)
   offset, spacing = get_forecast_offset_and_spacing(init, leads)
-  _common_axis(ds, TIME)
-  _common_axis(ds, DELTA)
+  _common_axis(forecast, TIME)
+  _common_axis(forecast, DELTA)
   if desired_time_dims == VALID_AND_DELTA:
     kept = leads[offset::spacing]
     times = np.unique(init[:, None] + kept[None, :])
@@ -275,14 +272,14 @@ def index_on_valid_time(forecast, *,
     rename = {TIME: INIT, DELTA: TIME}
     sizes = {INIT: init.size, TIME: times.size}
     coords = {INIT: xl.Coord((INIT,), init), TIME: xl.Coord((TIME,), times)}
-  coords.update(_other_coords(ds, (TIME, DELTA)))
-  out = xl.Dataset(coords=coords, attrs=ds.attrs)
-  for name, da in ds.items():
+  coords.update(_other_coords(forecast, (TIME, DELTA)))
+  out = xl.Dataset(coords=coords, attrs=forecast.attrs)
+  for name, da in forecast.items():
     dims = tuple(rename.get(d, d) for d in da.dims)
     data = _gather(da, dims, dict(da.sizes, **sizes), maps, np.float32,
                    allow_int=True)
     out[name] = xl.DataArray(data, dims, name=name, attrs=da.attrs)
-  return _public(forecast, out)
+  return out
 
 
 # ---- probabilistic climatological forecasts ----------------------------------------
@@ -473,6 +470,7 @@ def _check_time_spacing(times: np.ndarray, time_dim: str,
                        'resolution.')
 
 
+@xl.boundary
 def sample_forecasts_core(truth, sampled_init_times, output_init_times,
                           timedeltas, *, realization_name: str = REALIZATION,
                           time_dim: str = TIME, add_source_time: bool = False,
@@ -484,18 +482,17 @@ def sample_forecasts_core(truth, sampled_init_times, output_init_times,
   subset of a sampled table's columns with the matching output times.  With
   add_source_time, `source_time` (datetime64[ns]) holds the truth times read.
   A needed time the truth lacks raises ValueError listing the missing times."""
-  ds = xl.from_xarray(truth)
   sampled = np.asarray(sampled_init_times, dtype='datetime64[ns]')
   out_times = pd.DatetimeIndex(output_init_times).as_unit('ns')
   deltas = pd.TimedeltaIndex(timedeltas).as_unit('ns')
   if sampled.ndim != 2 or sampled.shape[1] != out_times.size:
     raise ValueError(f'sampled_init_times has shape {sampled.shape}; want '
                      f'(members, {out_times.size})')
-  if DELTA in ds.sizes:
+  if DELTA in truth.sizes:
     raise ValueError(f'INPUT_PATH data already had {DELTA} as a dimension')
   needed = (sampled[:, None, :] +
             deltas.values.astype('timedelta64[ns]')[None, :, None])
-  index = pd.Index(ds.coords[time_dim].values)
+  index = pd.Index(truth.coords[time_dim].values)
   missing = pd.to_datetime(np.unique(needed)).difference(index)
   if missing.size:
     raise ValueError(
@@ -508,13 +505,13 @@ def sample_forecasts_core(truth, sampled_init_times, output_init_times,
   sizes = {realization_name: sampled.shape[0], DELTA: deltas.size,
            time_dim: out_times.size}
   maps = {time_dim: (head, pos)}
-  coords = _other_coords(ds, (time_dim,))
+  coords = _other_coords(truth, (time_dim,))
   coords.update({realization_name: xl.Coord((realization_name,),
                                             np.arange(sampled.shape[0])),
                  DELTA: xl.Coord((DELTA,), deltas.values),
                  time_dim: xl.Coord((time_dim,), out_times.values)})
-  out = xl.Dataset(coords=coords, attrs=ds.attrs)
-  for name, da in ds.items():
+  out = xl.Dataset(coords=coords, attrs=truth.attrs)
+  for name, da in truth.items():
     if time_dim not in da.dims:
       raise ValueError(f'variable {name!r} has no {time_dim!r} dim to sample '
                        f'forecasts from (dims {da.dims})')
@@ -524,9 +521,10 @@ def sample_forecasts_core(truth, sampled_init_times, output_init_times,
     out[name] = xl.DataArray(data, dims, name=name, attrs=da.attrs)
   if add_source_time:
     out[SOURCE_TIME] = xl.DataArray(needed, head, name=SOURCE_TIME)
-  return _public(truth, out)
+  return out
 
 
+@xl.boundary
 def compute_probabilistic_climatological_forecasts(
     truth, *, initial_time_start: str, initial_time_end: str,
     climatology_start_year: int = 1990, climatology_end_year: int = 2020,
@@ -545,13 +543,13 @@ def compute_probabilistic_climatological_forecasts(
   forecast_duration (leads every timedelta_spacing from 0), each starting at
   a time from `get_sampled_init_times`.  Keyword arguments are the script's
   flags, with its defaults."""
-  ds = xl.from_xarray(truth)
   if variables:
-    ds = ds[[variables] if isinstance(variables, str) else list(variables)]
+    truth = truth[[variables] if isinstance(variables, str)
+                  else list(variables)]
   if levels:
-    ds = ds.isel(level=_positions(ds.coords['level'].values,
-                                  [int(l) for l in levels], 'level'))
-  _check_time_spacing(np.asarray(ds.coords[time_dim].values), time_dim,
+    truth = truth.isel(level=_positions(truth.coords['level'].values,
+                                        [int(l) for l in levels], 'level'))
+  _check_time_spacing(np.asarray(truth.coords[time_dim].values), time_dim,
                       timedelta_spacing, initial_time_spacing)
   ensemble_size = get_ensemble_size(
       ensemble_size, climatology_start_year, climatology_end_year,
@@ -560,7 +558,7 @@ def compute_probabilistic_climatological_forecasts(
                                     freq=initial_time_spacing)
   timedeltas = pd.timedelta_range('0 days', forecast_duration,
                                   freq=timedelta_spacing)
-  if DELTA in ds.sizes:
+  if DELTA in truth.sizes:
     raise ValueError(f'INPUT_PATH data already had {DELTA} as a dimension')
   sampled = get_sampled_init_times(
       output_init_times, climatology_start_year=climatology_start_year,
@@ -576,9 +574,8 @@ def compute_probabilistic_climatological_forecasts(
             f'sample_hold_days={sample_hold_days} means observations may be '
             'needed up to 1 year before/after the [CLIMATOLOGY_START_YEAR, '
             'CLIMATOLOGY_END_YEAR] interval.')
-  out = sample_forecasts_core(ds, sampled, output_init_times, timedeltas,
-                              realization_name=realization_name,
-                              time_dim=time_dim,
-                              add_source_time=add_source_time,
-                              missing_hint=hint)
-  return _public(truth, out)
+  return sample_forecasts_core(truth, sampled, output_init_times, timedeltas,
+                               realization_name=realization_name,
+                               time_dim=time_dim,
+                               add_source_time=add_source_time,
+                               missing_hint=hint)

@@ -125,10 +125,7 @@ def _coords(ds, time_dim: str, times, method: str) -> dict:
   return out
 
 
-def _public(obj, result):
-  return xl.to_xarray(result) if xl.is_native_xarray(obj) else result
-
-
+@xl.boundary
 def resample_in_time_core(chunk, method: str, period, statistic: str,
                           skipna: bool, *, time_dim: str = 'time',
                           label_side: str = 'left'):
@@ -137,30 +134,28 @@ def resample_in_time_core(chunk, method: str, period, statistic: str,
   (T - period, T] labelled T without the first bin (right); rolling output T
   reduces the `period // delta_t` steps ending at T."""
   period = pd.to_timedelta(period)
-  ds = xl.from_xarray(chunk)
-  if time_dim not in ds.coords:
+  if time_dim not in chunk.coords:
     raise KeyError(time_dim)
-  times, bins, window = _plan(ds.coords[time_dim].values, method, period,
+  times, bins, window = _plan(chunk.coords[time_dim].values, method, period,
                               label_side)
   if statistic not in STATISTICS:
     raise ValueError(f'Unhandled statistic={statistic!r}: one of {STATISTICS}')
-  coords = _coords(ds, time_dim, times, method)
-  if isinstance(ds, xl.DataArray):
-    if time_dim not in ds.dims:
+  coords = _coords(chunk, time_dim, times, method)
+  if isinstance(chunk, xl.DataArray):
+    if time_dim not in chunk.dims:
       return chunk
-    v = _stats(ds, time_dim, [statistic], skipna, bins, window)[statistic]
-    out = xl.DataArray(v, ds.dims, {k: c for k, c in coords.items()
-                                    if all(d in ds.dims for d in c.dims)},
-                       ds.name, ds.attrs)
-    return _public(chunk, out)
-  out = xl.Dataset(coords=coords, attrs=ds.attrs)
-  for name, da in ds.items():
+    v = _stats(chunk, time_dim, [statistic], skipna, bins, window)[statistic]
+    coords = {k: c for k, c in coords.items()
+              if all(d in chunk.dims for d in c.dims)}
+    return xl.DataArray(v, chunk.dims, coords, chunk.name, chunk.attrs)
+  out = xl.Dataset(coords=coords, attrs=chunk.attrs)
+  for name, da in chunk.items():
     if time_dim in da.dims:
       v = _stats(da, time_dim, [statistic], skipna, bins, window)[statistic]
       out[name] = xl.DataArray(v, da.dims, name=name, attrs=da.attrs)
     else:
       out[name] = da
-  return _public(chunk, out)
+  return out
 
 
 def _get_vars(list_of_vars, time_dependent_vars) -> list:
@@ -178,6 +173,7 @@ def _get_vars(list_of_vars, time_dependent_vars) -> list:
   return list_of_vars
 
 
+@xl.boundary
 def resample_in_time(ds, *, period, method: str = 'resample',
                      mean_vars: Sequence[str] = (),
                      min_vars: Sequence[str] = (),
@@ -195,8 +191,6 @@ def resample_in_time(ds, *, period, method: str = 'resample',
   [T, T + period) (left) or (T - period, T] (right), so resample and rolling
   agree at common times.  All statistics of a variable come from one read."""
   period = pd.to_timedelta(period)
-  src = ds
-  ds = xl.from_xarray(ds)
   if time_start is not None or time_stop is not None:
     index = pd.Index(ds.coords[time_dim].values)
     ds = ds.isel({time_dim: index.slice_indexer(time_start, time_stop)})
@@ -237,4 +231,4 @@ def resample_in_time(ds, *, period, method: str = 'resample',
       da = ds[name]
       out[key] = xl.DataArray(per_var[name][s], da.dims, name=key,
                               attrs=da.attrs)
-  return _public(src, out)
+  return out

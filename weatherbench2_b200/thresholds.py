@@ -132,9 +132,11 @@ def _materialise(clim_da: xl.DataArray, maps: dict) -> xl.DataArray:
 
 
 @dataclasses.dataclass
-class Threshold:
+class Threshold(xl.Boundary):
   """Threshold for discrete probabilistic metric evaluation
   (thresholds.py:92-115)."""
+
+  _boundary_methods = ('compute',)
 
   climatology: t.Any
   quantile: float
@@ -160,7 +162,6 @@ class QuantileThreshold(Threshold):
     return id(self)
 
   def compute(self, truth) -> xl.Dataset:
-    truth = xl.from_xarray(truth)
     clim = xl.from_xarray(self.climatology)
     variables = [str(k) for k in truth.keys()]
     clim_q = _get_climatology_quantile(clim, variables)
@@ -199,7 +200,6 @@ class GaussianQuantileThreshold(Threshold):
     return float(special.ndtri(self.quantile))  # == scipy.stats.norm.ppf
 
   def compute(self, truth) -> xl.Dataset:
-    truth = xl.from_xarray(truth)
     clim = xl.from_xarray(self.climatology)
     variables = [str(k) for k in truth.keys()]
     mean = _get_climatology_mean(clim, variables)

@@ -278,7 +278,7 @@ def _run(ds: xl.Dataset, plan, labels, hours, stats: Sequence[str]) -> dict:
   return out
 
 
-def _compute(obs, window_size: int, clim_years: slice,
+def _compute(ds, window_size: int, clim_years: slice,
              hours: Optional[Sequence[int]], method: int,
              stats: Sequence[str]) -> dict:
   """{stat: lite Dataset}; the daily fast mean averages the raw steps, every
@@ -286,7 +286,6 @@ def _compute(obs, window_size: int, clim_years: slice,
   _check_window(window_size)
   for s in stats:
     _check_stat(s)
-  ds = xl.from_xarray(obs)
   times = ds.coords['time'].values
   groups = [(list(stats), hours is None and method == EXPLICIT)]
   if hours is None and method == FAST:
@@ -341,14 +340,13 @@ def _run_quantile(ds: xl.Dataset, plan, labels, hours, spec) -> dict:
   return out
 
 
-def _compute_quantile(obs, window_size: int, clim_years: slice,
+def _compute_quantile(ds, window_size: int, clim_years: slice,
                       hours: Optional[Sequence[int]], spec) -> xl.Dataset:
   """The Quantile / SEEPSThreshold climatology, explicit method; the daily
   statistics take the daily resample (utils.py:127-140)."""
   _check_window(window_size)
   if not isinstance(spec, SEEPSThreshold):
     _quantile_values(spec.quantiles)
-  ds = xl.from_xarray(obs)
   if isinstance(spec, SEEPSThreshold) and spec.var not in ds:
     raise KeyError(spec.var)
   plan, labels = _plan(ds.coords['time'].values, clim_years, hours, EXPLICIT,
@@ -362,56 +360,56 @@ def _compute_quantile(obs, window_size: int, clim_years: slice,
                     attrs=ds.attrs)
 
 
-def _public(obs, result: xl.Dataset):
-  return xl.to_xarray(result) if xl.is_native_xarray(obs) else result
-
-
 def _hours(hour_interval: int):
   return list(range(0, 24, hour_interval))
 
 
+@xl.boundary
 def compute_hourly_stat(obs, window_size: int, clim_years: slice,
                         hour_interval: int, stat_fn: StatFn = 'mean'):
   """Climatology by hour of day and day of year, `explicit` method."""
   spec = _quantile_spec(stat_fn)
   if spec is not None:
-    return _public(obs, _compute_quantile(obs, window_size, clim_years,
-                                          _hours(hour_interval), spec))
+    return _compute_quantile(obs, window_size, clim_years,
+                             _hours(hour_interval), spec)
   _check_stat(stat_fn)
   res = _compute(obs, window_size, clim_years, _hours(hour_interval), EXPLICIT,
                  [stat_fn])
-  return _public(obs, res[stat_fn])
+  return res[stat_fn]
 
 
+@xl.boundary
 def compute_daily_stat(obs, window_size: int, clim_years: slice,
                        stat_fn: StatFn = 'mean'):
   """Climatology by day of year of the daily means, `explicit` method."""
   spec = _quantile_spec(stat_fn)
   if spec is not None:
-    return _public(obs, _compute_quantile(obs, window_size, clim_years, None,
-                                          spec))
+    return _compute_quantile(obs, window_size, clim_years, None, spec)
   _check_stat(stat_fn)
   res = _compute(obs, window_size, clim_years, None, EXPLICIT, [stat_fn])
-  return _public(obs, res[stat_fn])
+  return res[stat_fn]
 
 
+@xl.boundary
 def compute_hourly_stat_fast(obs, window_size: int, clim_years: slice,
                              hour_interval: int, stat_fn: str = 'mean'):
   """Per-day mean / std by hour of day, smoothed over the window (`fast`)."""
   _check_stat(stat_fn)
   res = _compute(obs, window_size, clim_years, _hours(hour_interval), FAST,
                  [stat_fn])
-  return _public(obs, res[stat_fn])
+  return res[stat_fn]
 
 
+@xl.boundary
 def compute_daily_stat_fast(obs, window_size: int, clim_years: slice,
                             stat_fn: str = 'mean'):
   """Per-day mean (raw steps) / std (daily means), smoothed (`fast`)."""
   _check_stat(stat_fn)
   res = _compute(obs, window_size, clim_years, None, FAST, [stat_fn])
-  return _public(obs, res[stat_fn])
+  return res[stat_fn]
 
 
+@xl.boundary
 def compute_climatology(obs, *, frequency: str = 'hourly',
                         hour_interval: int = 1, window_size: int = 61,
                         start_year: int = 1990, end_year: int = 2020,
@@ -451,8 +449,7 @@ def compute_climatology(obs, *, frequency: str = 'hourly',
   res = (_compute(obs, window_size, years, hours,
                   EXPLICIT if method == 'explicit' else FAST, moments)
          if moments else {})
-  ds = xl.from_xarray(obs)
-  out = xl.Dataset(attrs=ds.attrs)
+  out = xl.Dataset(attrs=obs.attrs)
   for s in stats:
     if s == 'quantile':
       q = _compute_quantile(obs, window_size, years, hours,
@@ -470,4 +467,4 @@ def compute_climatology(obs, *, frequency: str = 'hourly',
         key = name if s == 'mean' else f'{name}_{s}'
         da.name = key
         out[key] = da
-  return _public(obs, out)
+  return out

@@ -6,8 +6,8 @@ the build or GPU boxes, so the drop-in operators of this package work on this
 small stand-in, which implements exactly the subset of the xarray API the hot
 path and its callers use: named dims, coordinate lookup, broadcasting
 arithmetic by dimension name, `mean(dim, skipna)`, `isel/sel`, `expand_dims`,
-`concat`, `merge`.  When real xarray IS importable the public entry points
-convert at the boundary (`from_xarray` / `to_xarray`).
+`concat`, `merge`.  The public entry points also take real xarray objects:
+`boundary` converts them on the way in and the result on the way out.
 
 `data` may be a NumPy array (host) or a `torch.Tensor` on a CUDA device; the
 metric operators read it in place either way.  Everything the container itself
@@ -15,6 +15,7 @@ computes (results are tiny) is NumPy.
 """
 from __future__ import annotations
 
+import functools
 import numbers
 from typing import Any, Iterable, Mapping, Optional, Sequence
 
@@ -943,6 +944,49 @@ def to_xarray(obj):
 
 def is_native_xarray(obj) -> bool:
   return type(obj).__module__.startswith('xarray')
+
+
+def _lite(obj):
+  return from_xarray(obj) if is_native_xarray(obj) else obj
+
+
+def boundary(fn):
+  """Lets `fn`, written for lite containers, take native xarray objects too.
+
+  Every native argument, positional or keyword, is converted with
+  `from_xarray` before the call.  If the first container argument (native or
+  lite) was native, a lite Dataset or DataArray result is converted with
+  `to_xarray`; any other result passes through.  A call with lite arguments
+  converts nothing, so operators that call each other convert only at the
+  outermost call."""
+
+  @functools.wraps(fn)
+  def call(*args, **kwargs):
+    values = args + tuple(kwargs.values())
+    if not any(is_native_xarray(a) for a in values):
+      return fn(*args, **kwargs)
+    first = next(a for a in values
+                 if isinstance(a, (Dataset, DataArray)) or is_native_xarray(a))
+    out = fn(*map(_lite, args), **{k: _lite(v) for k, v in kwargs.items()})
+    if is_native_xarray(first) and isinstance(out, (Dataset, DataArray)):
+      return to_xarray(out)
+    return out
+
+  return call
+
+
+class Boundary:
+  """Base class that puts `boundary` on the methods named in
+  `_boundary_methods`, in the class that names them and in every subclass
+  that overrides one."""
+
+  _boundary_methods: tuple = ()
+
+  def __init_subclass__(cls, **kwargs):
+    super().__init_subclass__(**kwargs)
+    for name in cls._boundary_methods:
+      if name in cls.__dict__:
+        setattr(cls, name, boundary(cls.__dict__[name]))
 
 
 class LazyGather(DataArray):
