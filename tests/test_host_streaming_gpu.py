@@ -102,6 +102,74 @@ def test_det_host_chunk_sweep_with_slab_cache(small_stage_ctx, cache_slabs):
     assert st['cache_misses'] > 0  # thrashing, but still correct
 
 
+def _ens_device(ctx, x, t, m, member_stride, off_x, off_t, spec, skipna):
+  """Reference result: the same operands uploaded whole, device entry."""
+  from weatherbench2_b200 import _lib
+  dx, dt_ = ctx.to_device(x), ctx.to_device(t)
+  base = min(dx, dt_)
+  n = off_x.size
+  out = ctx.malloc(n * _lib.ENS_NSTAT * 8)
+  try:
+    ctx.ens_metrics(base, base, _lib.F32, m, member_stride,
+                    off_x + (dx - base) // 4, off_t + (dt_ - base) // 4, spec,
+                    skipna, out)
+    return ctx.from_device(out, (n, 1, _lib.ENS_NSTAT), np.float64)
+  finally:
+    for p in (dx, dt_, out):
+      ctx.free(p)
+
+
+@pytest.mark.parametrize('cache_slabs', [0, 7, 1000])
+def test_ens_host_chunk_sweep_with_slab_cache(small_stage_ctx, cache_slabs):
+  """The ensemble twin of the sweep above: truth slabs repeat from chunk to
+  chunk.  20 members fill 1 MiB staging with 5 fields, so a chunk of 12 fields
+  runs in three groups.  With cache_slabs = 7, groups evict truth slots that
+  the previous group read, so their cache fills wait for its kernel."""
+  from weatherbench2_b200 import _lib
+  ctx = small_stage_ctx
+  m, nlat, nlon, nlead, nlev, ninit = 20, 33, 64, 4, 3, 5
+  slab = nlat * nlon
+  nf = nlead * nlev
+  _, _, spec = _weights(ctx, nlat, nlon)
+  rs = np.random.RandomState(4)
+  ntime = ninit + nlead
+  truth = rs.standard_normal((ntime, nlev, nlat, nlon)).astype(np.float32)
+  slab_bytes = (slab + 63) // 64 * 64 * 4
+  ctx.set_slab_cache(cache_slabs * slab_bytes)
+  ctx.reset_transfer_stats()
+  h2d = []
+  try:
+    for i in range(ninit):
+      x = rs.standard_normal((m, nlead, nlev, nlat, nlon)).astype(np.float32)
+      if i == 2:
+        x[7, 1, 0, 3, 5] = np.nan
+      off_x = np.arange(nf, dtype=np.int64) * slab
+      lead_t = (i + np.arange(nlead))[:, None] * nlev + np.arange(nlev)[None]
+      off_t = (lead_t * slab).ravel().astype(np.int64)
+      got = np.empty((nf, 1, _lib.ENS_NSTAT), np.float64)
+      before = ctx.transfer_stats()['h2d_bytes']
+      ctx.ens_metrics_host(x.ctypes.data, truth.ctypes.data, m, nf * slab,
+                           off_x, off_t, spec, False, got.ctypes.data)
+      h2d.append(ctx.transfer_stats()['h2d_bytes'] - before)
+      want = _ens_device(ctx, x, truth, m, nf * slab, off_x, off_t, spec,
+                         False)
+      np.testing.assert_array_equal(got, want)
+    st = ctx.transfer_stats()
+  finally:
+    ctx.set_slab_cache(0)
+  full = (m + 1) * nf * slab * 4
+  if cache_slabs == 0:
+    assert all(b == full for b in h2d) and st['cache_hits'] == 0
+  elif cache_slabs == 1000:
+    # first chunk ships everything, later ones the members + one new valid time
+    assert h2d[0] == full
+    assert all(b == (m * nlead + 1) * nlev * slab * 4 for b in h2d[1:])
+    assert st['cache_hits'] == (ninit - 1) * (nlead - 1) * nlev
+    assert st['cache_misses'] == (nlead + ninit - 1) * nlev
+  else:
+    assert st['cache_misses'] > 0  # thrashing, but still correct
+
+
 def test_ens_host_matches_device_entry_and_oracle(small_stage_ctx):
   from weatherbench2_b200 import _lib
   ctx = small_stage_ctx
