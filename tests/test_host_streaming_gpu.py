@@ -210,7 +210,7 @@ def test_ens_host_matches_device_entry_and_oracle(small_stage_ctx):
                              rtol=1e-5)
 
 
-def test_regrid_host_is_bit_identical_to_device_entry(small_stage_ctx):
+def test_regrid_conservative_host_is_bit_identical_to_device_entry(small_stage_ctx):
   from weatherbench2_b200 import regridding as rg
   ctx = small_stage_ctx
   src = rg.Grid.from_degrees(np.linspace(0, 360, 72, endpoint=False),
@@ -223,7 +223,9 @@ def test_regrid_host_is_bit_identical_to_device_entry(small_stage_ctx):
   x = rs.standard_normal((nf, 72, 37)).astype(np.float32)
   x[5, 10:14, 3:9] = np.nan
   got = np.empty((nf, 24, 13), np.float32)
-  assert r.regrid_host(ctx, x.ctypes.data, got.ctypes.data, nf)
+  lon_w, lat_w = r._weights  # pylint: disable=protected-access
+  ctx.regrid_conservative_host(x.ctypes.data, got.ctypes.data, nf, 72 * 37,
+                               24 * 13, lon_w, lat_w)
   dsrc = ctx.to_device(x)
   ddst = ctx.malloc(nf * 24 * 13 * 4)
   try:

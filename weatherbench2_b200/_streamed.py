@@ -1,17 +1,15 @@
 """Where an operator's data lives decides how its C entry runs: the one
 residency rule of the operators, in two forms.
 
-The quantile, average, time-window, precipitation-accumulation and
-climatology operators each have an entry pair in `_lib.Context`:
-`X(x, dtype, *args, *outputs)` reads device addresses, and
-`X_host(x, dtype, *args, budget, *outputs)` streams host memory through the
-device in bands whose device footprint stays within `budget` bytes.  `run`
-holds the rule that picks between them.
-
-The derived-variable, ensemble-mean, spectrum-interpolation and staged regrid
-operators have only the device entry.  `run_whole` runs it on CUDA operands
-in place, and otherwise uploads the host operands whole and copies the results
-back.  Either way each operator only computes its layout."""
+`place` serves the operators with an entry pair in `_lib.Context`, a device
+entry and a `_host` twin that streams host memory through the device: the
+zonal spectrum and the conservative regridder directly, and the quantile,
+average, time-window, precipitation-accumulation and climatology operators
+through `run`.  The derived-variable, ensemble-mean, spectrum-interpolation
+and nearest and bilinear regrid operators have only the device entry:
+`run_whole` runs it on CUDA operands in place, and otherwise uploads the host
+operands whole and copies the results back.  Either way each operator only
+computes its layout."""
 from __future__ import annotations
 
 import functools
@@ -31,6 +29,37 @@ def _torch_dtype(dtype):
   microseconds, as long as the rest of a small call)."""
   import torch  # pylint: disable=import-outside-toplevel
   return getattr(torch, np.dtype(dtype).name)
+
+
+def place(data, outputs: Sequence, device, host, *,
+          perm: Optional[Sequence[int]] = None, dtype=None) -> list:
+  """The placement half of `run`, for any entry pair: lays out `data` (a
+  variable's `.data`) and allocates the outputs as `run` describes, runs
+  `device(x, code, *outs)` on a CUDA tensor and `host(x, code, *outs)` on
+  anything else, and returns the outputs in order.  `code` is the entry's
+  dtype code of `x`.  The arms get arrays rather than addresses, so that a
+  device arm can initialise an output on torch's current stream; an output
+  not asked for is None.  When every output asked for is empty no arm runs."""
+  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
+    import torch  # pylint: disable=import-outside-toplevel
+    x = data if perm is None else data.permute(*perm)
+    x = (x if dtype is None else x.to(_torch_dtype(dtype))).contiguous()
+    code = _lib.F64 if x.dtype == torch.float64 else _lib.F32
+    res = [None if o is None else
+           torch.empty(o[0], dtype=_torch_dtype(o[1]), device=x.device)
+           for o in outputs]
+    arm = device
+  else:
+    x = xl._np(data)  # pylint: disable=protected-access
+    x = np.ascontiguousarray(x if perm is None else np.transpose(x, perm),
+                             dtype=dtype)
+    code = _lib.F64 if x.dtype == np.float64 else _lib.F32
+    ctx = _lib.default_context()
+    res = [None if o is None else ctx.pinned_result(*o) for o in outputs]
+    arm = host
+  if any(math.prod(o[0]) for o in outputs if o is not None):
+    arm(x, code, *res)
+  return res
 
 
 def run(entry: str, data, args: Sequence, outputs: Sequence, budget: int, *,
@@ -54,27 +83,16 @@ def run(entry: str, data, args: Sequence, outputs: Sequence, budget: int, *,
   and which is returned as None.  `kwargs` go to the entry as they are.
   When every output asked for is empty the entry is not called."""
   ctx = _lib.default_context()
-  if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-    import torch  # pylint: disable=import-outside-toplevel
-    x = data if perm is None else data.permute(*perm)
-    x = (x if dtype is None else x.to(_torch_dtype(dtype))).contiguous()
-    code = _lib.F64 if x.dtype == torch.float64 else _lib.F32
-    res = [None if o is None else
-           torch.empty(o[0], dtype=_torch_dtype(o[1]), device=x.device)
-           for o in outputs]
-    fn, extra, ptr = getattr(ctx, entry), (), lambda a: a.data_ptr()
-  else:
-    x = xl._np(data)  # pylint: disable=protected-access
-    x = np.ascontiguousarray(x if perm is None else np.transpose(x, perm),
-                             dtype=dtype)
-    code = _lib.F64 if x.dtype == np.float64 else _lib.F32
-    res = [None if o is None else ctx.pinned_result(*o) for o in outputs]
-    fn, extra, ptr = (getattr(ctx, entry + '_host'), (budget,),
-                      lambda a: a.ctypes.data)
-  if any(math.prod(o[0]) for o in outputs if o is not None):
-    fn(ptr(x), code, *args, *extra,
-       *[None if a is None else ptr(a) for a in res], **kwargs)
-  return res
+
+  def device(x, code, *res):
+    getattr(ctx, entry)(x.data_ptr(), code, *args, *[
+        None if a is None else a.data_ptr() for a in res], **kwargs)
+
+  def host(x, code, *res):
+    getattr(ctx, entry + '_host')(x.ctypes.data, code, *args, budget, *[
+        None if a is None else a.ctypes.data for a in res], **kwargs)
+
+  return place(data, outputs, device, host, perm=perm, dtype=dtype)
 
 
 def run_whole(datas: Sequence, outputs: Sequence, call, *,

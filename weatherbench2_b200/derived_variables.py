@@ -87,6 +87,25 @@ class ZonalEnergySpectrum(DerivedVariable):
     return xl.DataArray(self._circumference(lat) * diffs[0] / 360,
                         ('latitude',), {'latitude': lat})
 
+  @staticmethod
+  def _layout(da, sum_dim):
+    """`da` as (outer..., latitude, longitude), `sum_dim` first so that field i
+    adds to result slot i % nout; the result's outer dims and shape, nfield,
+    the length of `sum_dim` (1 without it) and nout."""
+    outer = tuple(d for d in da.dims if d not in ('latitude', 'longitude'))
+    if sum_dim is not None:
+      if sum_dim not in outer:
+        raise ValueError(f'{sum_dim!r} is not a dimension of the data')
+      outer = (sum_dim,) + tuple(d for d in outer if d != sum_dim)
+    work = da.transpose(*(outer + ('latitude', 'longitude')))
+    oshape = tuple(work.sizes[d] for d in outer)
+    nfield = int(np.prod(oshape))  # 1 without outer dims
+    nt = oshape[0] if sum_dim is not None else 1
+    nout = nfield // nt
+    if sum_dim is not None:
+      outer, oshape = outer[1:], oshape[1:]
+    return work, outer, oshape, nfield, nt, nout
+
   def compute(self, dataset, time_sum_dim: t.Optional[str] = None):
     """Zonal power at wavenumber and frequency (derived_variables.py:592-626).
 
@@ -101,43 +120,26 @@ class ZonalEnergySpectrum(DerivedVariable):
     lon = dataset['longitude'].values
     if 'latitude' not in da.dims or 'longitude' not in da.dims:
       raise ValueError(f'{self.variable_name} needs latitude and longitude')
-    outer = tuple(d for d in da.dims if d not in ('latitude', 'longitude'))
-    if time_sum_dim is not None:
-      if time_sum_dim not in outer:
-        raise ValueError(f'{time_sum_dim!r} is not a dimension of the data')
-      outer = (time_sum_dim,) + tuple(d for d in outer if d != time_sum_dim)
-    work = da.transpose(*(outer + ('latitude', 'longitude')))
-    data = work.data
+    work, out_outer, oshape, nfield, _, nout = self._layout(da, time_sum_dim)
     ctx = _lib.default_context()
     nlat, nlon = lat.size, lon.size
     nk = nlon // 2 + 1
-    oshape = tuple(work.sizes[d] for d in outer)
-    nfield = int(np.prod(oshape)) if oshape else 1
     scale = self._circumference(lat)
-    nt = oshape[0] if time_sum_dim is not None else 1
-    nout = nfield // nt
-    res_shape = (oshape[1:] if time_sum_dim is not None else oshape) + (nlat,
-                                                                        nk)
-    is_torch = xl._is_torch(data)  # pylint: disable=protected-access
-    if is_torch and data.is_cuda:
-      import torch  # pylint: disable=import-outside-toplevel
-      x = data.to(torch.float32).contiguous()
-      out = torch.zeros(res_shape, device=data.device, dtype=torch.float32)
+    summed = time_sum_dim is not None
+
+    def device(x, _, out):
+      if summed:  # the device entry adds into `out`
+        out.zero_()
       ctx.zonal_spectrum(x.data_ptr(), nfield, nlat, nlon, scale,
-                         out.data_ptr(), time_sum_dim is not None, nout)
-      values = out
-    else:
-      # host data: streamed through double-buffered staging; with a time sum
-      # the accumulator stays in HBM and only the sum comes back
-      x = np.ascontiguousarray(np.asarray(data), dtype=np.float32)
-      values = ctx.pinned_result(res_shape, np.float32)  # overwritten below
-      if not nfield:
-        values[...] = 0
-      if nfield:
-        ctx.zonal_spectrum_host(x.ctypes.data, nfield, nlat, nlon, scale,
-                                values.ctypes.data, time_sum_dim is not None,
-                                nout)
-    out_outer = outer[1:] if time_sum_dim is not None else outer
+                         out.data_ptr(), summed, nout)
+
+    # host data is streamed through double-buffered staging; with a time sum
+    # the accumulator stays in HBM and only the sum comes back
+    values, = _streamed.place(
+        work.data, [(oshape + (nlat, nk), np.float32)], device,
+        lambda x, _, out: ctx.zonal_spectrum_host(
+            x.ctypes.data, nfield, nlat, nlon, scale, out.ctypes.data, summed,
+            nout), dtype=np.float32)
     dims = out_outer + ('latitude', 'zonal_wavenumber')
     base_frequency = np.fft.rfftfreq(nlon)  # derived_variables.py:614
     with np.errstate(divide='ignore'):
@@ -155,7 +157,7 @@ class ZonalEnergySpectrum(DerivedVariable):
     ref_dims = tuple(d for d in da.dims if d != 'longitude' and
                      d != time_sum_dim) + ('zonal_wavenumber',)
     result = xl.DataArray(values, dims, coords, self.variable_name)
-    if not is_torch:
+    if not xl._is_torch(work.data):  # pylint: disable=protected-access
       result = result.transpose(*ref_dims)
     return result
 
@@ -176,19 +178,10 @@ class ZonalEnergySpectrum(DerivedVariable):
     da = dataset[self.variable_name]
     lat = dataset['latitude'].values
     lon = dataset['longitude'].values
-    outer = tuple(d for d in da.dims if d not in ('latitude', 'longitude'))
-    if time_mean_dim is not None:
-      if time_mean_dim not in outer:
-        raise ValueError(f'{time_mean_dim!r} is not a dimension of the data')
-      outer = (time_mean_dim,) + tuple(d for d in outer if d != time_mean_dim)
-    work = da.transpose(*(outer + ('latitude', 'longitude')))
-    data = work.data
+    work, out_outer, oshape, nfield, nt, nout = self._layout(da,
+                                                             time_mean_dim)
     nlat, nlon = lat.size, lon.size
     nk = nlon // 2 + 1
-    oshape = tuple(work.sizes[d] for d in outer)
-    nfield = int(np.prod(oshape)) if oshape else 1
-    nt = oshape[0] if time_mean_dim is not None else 1
-    nout = nfield // nt
     w = sp.lat_weights(lat)
     if lat_slice is not None:
       lo = -np.inf if lat_slice.start is None else lat_slice.start
@@ -197,21 +190,14 @@ class ZonalEnergySpectrum(DerivedVariable):
     if not w.sum() > 0:
       raise ValueError('the latitude band selects no latitude')
     scale = self._circumference(lat) * w / w.sum() / nt
-    res_shape = (oshape[1:] if time_mean_dim is not None else oshape) + (nk,)
     ctx = _lib.default_context()
-    if xl._is_torch(data) and data.is_cuda:  # pylint: disable=protected-access
-      import torch  # pylint: disable=import-outside-toplevel
-      x = data.to(torch.float32).contiguous()
-      out = torch.empty(res_shape, device=x.device, dtype=torch.float32)
-      ctx.zonal_spectrum_latsum(x.data_ptr(), nfield, nlat, nlon, scale,
-                                out.data_ptr(), nout)
-      values = out
-    else:
-      x = np.ascontiguousarray(np.asarray(data), dtype=np.float32)
-      values = np.empty(res_shape, dtype=np.float32)
-      ctx.zonal_spectrum_latsum_host(x.ctypes.data, nfield, nlat, nlon, scale,
-                                     values.ctypes.data, nout)
-    out_outer = outer[1:] if time_mean_dim is not None else outer
+    values, = _streamed.place(
+        work.data, [(oshape + (nk,), np.float32)],
+        lambda x, _, out: ctx.zonal_spectrum_latsum(
+            x.data_ptr(), nfield, nlat, nlon, scale, out.data_ptr(), nout),
+        lambda x, _, out: ctx.zonal_spectrum_latsum_host(
+            x.ctypes.data, nfield, nlat, nlon, scale, out.ctypes.data, nout),
+        dtype=np.float32)
     dims = out_outer + ('zonal_wavenumber',)
     coords = {k: c for k, c in work.coords.items()
               if all(d in out_outer for d in c.dims)}

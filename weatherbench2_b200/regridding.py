@@ -231,36 +231,24 @@ class Regridder:
     """Raw device-pointer entry: `nfield` float32 slabs (lon, lat) -> slabs."""
     raise NotImplementedError
 
-  def regrid_array(self, field):
-    """(..., lon, lat) -> (..., lon_target, lat_target), float32 like the
-    reference (JAX default).  NumPy in -> NumPy out; CUDA tensor in -> out."""
-    ctx = _lib.default_context()
-    is_torch = xl._is_torch(field)  # pylint: disable=protected-access
+  def _fields(self, field) -> tuple[int, tuple]:
+    """The field count and result shape of `field`, (..., lon, lat)."""
     shape = tuple(field.shape)
     if shape[-2:] != self.source.shape:
       raise ValueError(f'expected trailing dims {self.source.shape}, got '
                        f'{shape[-2:]}')
     batch = shape[:-2]
-    nfield = int(np.prod(batch)) if batch else 1
-    tshape = batch + self.target.shape
-    x = field
-    if not (is_torch and field.is_cuda):
-      x = np.ascontiguousarray(np.asarray(field), dtype=np.float32)
-      out = ctx.pinned_result(tshape, np.float32)
-      if nfield and self.regrid_host(ctx, x.ctypes.data, out.ctypes.data,
-                                     nfield):
-        return out  # streamed: H2D, kernel and D2H of neighbouring groups overlap
+    return int(np.prod(batch)), batch + self.target.shape
+
+  def regrid_array(self, field):
+    """(..., lon, lat) -> (..., lon_target, lat_target), float32 like the
+    reference (JAX default).  NumPy in -> NumPy out; CUDA tensor in -> out."""
+    ctx = _lib.default_context()
+    nfield, tshape = self._fields(field)
     return _streamed.run_whole(
-        [x], [(tshape, np.float32)],
+        [field], [(tshape, np.float32)],
         lambda i, o: self.regrid_device(ctx, i[0], o[0], nfield),
         dtype=np.float32)[0]
-
-  def regrid_host(self, ctx: _lib.Context, src_ptr: int, dst_ptr: int,
-                  nfield: int) -> bool:
-    """Host-pointer entry (double-buffered streaming); False = not available
-    for this regridder (the caller stages whole arrays instead)."""
-    del ctx, src_ptr, dst_ptr, nfield
-    return False
 
   @xl.boundary
   def regrid_dataset(self, dataset):
@@ -316,14 +304,20 @@ class ConservativeRegridder(Regridder):
     ctx.regrid_conservative(src_ptr, dst_ptr, nfield, src_stride or ns,
                             dst_stride or nt, lon_w, lat_w)
 
-  def regrid_host(self, ctx: _lib.Context, src_ptr: int, dst_ptr: int,
-                  nfield: int) -> bool:
-    lon_w, lat_w = self._weights
+  def regrid_array(self, field):
+    """As `Regridder.regrid_array`; NumPy input is streamed, so that the
+    copies and kernels of neighbouring field groups overlap."""
+    ctx = _lib.default_context()
+    nfield, tshape = self._fields(field)
     ns = self.source.shape[0] * self.source.shape[1]
     nt = self.target.shape[0] * self.target.shape[1]
-    ctx.regrid_conservative_host(src_ptr, dst_ptr, nfield, ns, nt, lon_w,
-                                 lat_w)
-    return True
+    return _streamed.place(
+        field, [(tshape, np.float32)],
+        lambda x, _, out: self.regrid_device(ctx, x.data_ptr(),
+                                             out.data_ptr(), nfield),
+        lambda x, _, out: ctx.regrid_conservative_host(
+            x.ctypes.data, out.ctypes.data, nfield, ns, nt, *self._weights),
+        dtype=np.float32)[0]
 
 
 # Nearest / bilinear regridders live in _regrid_interp.py (they need Regridder).
